@@ -86,7 +86,11 @@ EXPORTS = ["c2b_create", "c2b_destroy", "c2b_last_error", "c2b_configure", "c2b_
            "c2b_fastq_seqs", "c2b_fastq_offsets", "c2b_fastq_counts", "c2b_fastq_first_index", "c2b_fastq_free",
            "c2b_fastq_last_error", "c2b_fastq_filter", "c2b_fastq_filter_pair", "c2b_rc_merge_weights", "c2b_screen_reads", "c2b_serial_stats",
            "c2b_consensus_from_pairs", "c2b_alleles_build", "c2b_alleles_free", "c2b_alleles_n", "c2b_alleles_order", "c2b_alleles_arena", "c2b_alleles_offsets",
-           "c2b_alleles_lengths", "c2b_alleles_write_tsv", "c2b_alleles_around_cut", "c2b_alleles_cut_width", "c2b_alleles_cut_fetch"]
+           "c2b_alleles_lengths", "c2b_alleles_write_tsv", "c2b_alleles_around_cut", "c2b_alleles_cut_width", "c2b_alleles_cut_fetch",
+           "c2b_annotate_build", "c2b_annotate_free", "c2b_annotate_n", "c2b_annotate_arena", "c2b_annotate_offsets",
+           "c2b_annotate_cigar_arena", "c2b_annotate_cigar_offsets", "c2b_annotate_flags", "c2b_annotate_mapq", "c2b_annotate_first",
+           "c2b_annotate_last_record", "c2b_annotate_record_arena", "c2b_annotate_record_offsets", "c2b_annotate_write_fastq",
+           "c2b_annotate_write_sam"]
 
 _cache = {}
 
@@ -221,5 +225,22 @@ def load(path=None):
     L.c2b_alleles_cut_width.argtypes = [vp]
     L.c2b_alleles_cut_fetch.restype = C.c_int
     L.c2b_alleles_cut_fetch.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
+    cpp = C.POINTER(C.c_char_p)
+    L.c2b_annotate_build.restype = C.c_int
+    L.c2b_annotate_build.argtypes = [vp, vp, vp, i64, vp, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, i32, cpp, vp, i32, cpp, cpp, vp,
+                                     vp, C.c_uint32, i64, C.POINTER(vp)]
+    L.c2b_annotate_free.restype = None
+    L.c2b_annotate_free.argtypes = [vp]
+    L.c2b_annotate_n.restype = i64
+    L.c2b_annotate_n.argtypes = [vp]
+    for name in ("c2b_annotate_arena", "c2b_annotate_offsets", "c2b_annotate_cigar_arena", "c2b_annotate_cigar_offsets",
+                 "c2b_annotate_flags", "c2b_annotate_mapq", "c2b_annotate_first", "c2b_annotate_last_record",
+                 "c2b_annotate_record_arena", "c2b_annotate_record_offsets"):
+        getattr(L, name).restype = vp
+        getattr(L, name).argtypes = [vp]
+    L.c2b_annotate_write_fastq.restype = C.c_int
+    L.c2b_annotate_write_fastq.argtypes = [vp, vp, vp, i64, C.c_char_p, C.c_char_p, i32]
+    L.c2b_annotate_write_sam.restype = C.c_int
+    L.c2b_annotate_write_sam.argtypes = [vp, vp, vp, i64, C.c_char_p, C.c_char_p, C.c_char_p, i32, cpp, cpp, vp, i32]
     _cache[path] = L
     return L

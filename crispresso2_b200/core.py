@@ -204,13 +204,12 @@ def _variant_from(res, i, seq, ref_names, refs):
     for r in range(nref):
         s1, s2 = L.pair(i, r, alns[r][_A_ALNLEN])
         details.append((ref_names[r], s1, s2, scores[r]))
-    v = {"count": 1, "aln_scores": scores, "ref_aln_details": details}
     if best_milli <= 0:
-        v["best_match_score"] = -1
-        return v
+        return {"count": 1, "aln_scores": scores, "ref_aln_details": details, "best_match_score": -1}
     winners = [r for r in range(nref) if (winner_mask >> r) & 1]
-    v["aln_ref_names"] = [ref_names[r] for r in winners]
-    v["best_match_score"] = best_milli / 1000.0
+    # key order of CRISPRessoCORE.py:711-715
+    v = {"count": 1, "aln_ref_names": [ref_names[r] for r in winners], "aln_scores": scores, "ref_aln_details": details,
+         "best_match_score": best_milli / 1000.0}
     labels = []
     for r in winners:
         a = alns[r]
@@ -629,6 +628,7 @@ def _process_uniques(engine, buf, off, counts, keys, variantCache, ref_names, re
         st["N_CACHED_NOTALN"] += cb - n_bad
     src = lazy.BatchSource(None, keys_g, ref_names, refs, counts_g, parts=parts)
     src.weights, src.flags, src.lib_path, src.scaffold = weights, flags, engine.lib_path, scaffold
+    src.engine, src.packed_all, src.good = engine, (buf, off), (good if n_bad else None)     # annotate.py
     _sources[id(variantCache)] = src
     cls = src.lazy_class()
     not_aligned = {}

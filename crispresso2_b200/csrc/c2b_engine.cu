@@ -23,6 +23,8 @@
 
 #include "c2b_core.cuh"
 #include "c2b_split.cuh"
+#include "c2b_annotate.cuh"
+#include "c2b_fastq_int.h"
 
 using namespace c2b;
 
@@ -1501,6 +1503,175 @@ int c2b_classify_aligned_flags(c2b_engine *e, const char *read_al, const char *r
     rt_free(d_ops.p); rt_free(d_n.p);
     return rc;
 }
+
+// Read annotations (c2b_annotate.cuh) for unique reads in chunks: the chunk's inputs go up through one pinned buffer, a size
+// pass, a scan and a write pass run on the engine's stream, the texts come back through a second pinned buffer.  Device memory
+// is bounded by the chunk, whatever the number of reads.
+int c2b_annotate_build(c2b_engine *e, const uint8_t *reads, const int64_t *offsets, int64_t n_unique, const int32_t *bidx,
+                       int32_t R, int32_t NW, int32_t edit_cap, const c2b_read_rec *recs, const c2b_aln_rec *alns,
+                       const uint64_t *ops, const uint32_t *meta, const c2b_edit *edits,
+                       const uint32_t *amask, const int16_t *aname, const int32_t *label,
+                       int32_t n_names, const char *const *names, const uint8_t *name_rev,
+                       int32_t n_labels, const char *const *labels,
+                       const char *const *ref_seqs, const int32_t *ref_lens, const uint8_t *comp256, uint32_t flags,
+                       int64_t chunk, c2b_annotation **out)
+{
+    if (!e || !out || n_unique < 0 || (n_unique && (!offsets || !bidx)) || R < 1 || R > C2B_MAX_REFS || NW < 1 || edit_cap < 0 ||
+        n_names < R || !names || !name_rev || n_labels < 0 || (n_labels && !labels) || !ref_seqs || !ref_lens || !comp256)
+        return fail(e, C2B_E_ARG, "c2b_annotate_build: bad argument");
+    *out = nullptr;
+    int64_t nb = 0;                                               // batch reads referenced
+    for (int64_t u = 0; u < n_unique; u++) if (bidx[u] >= 0) nb = std::max<int64_t>(nb, (int64_t)bidx[u] + 1);
+    if (nb && (!recs || !alns || !ops || !meta || !amask || !aname || !label || (edit_cap && !edits)))
+        return fail(e, C2B_E_ARG, "c2b_annotate_build: batch arrays missing");
+    for (int64_t k = 0; k < nb; k++) {
+        if (label[k] < -1 || label[k] >= n_labels || aname[k] >= n_names) return fail(e, C2B_E_ARG, "c2b_annotate_build: label / name id out of range");
+        if (amask[k] && label[k] < 0) return fail(e, C2B_E_ARG, "c2b_annotate_build: aligned read without a class label");
+        if (amask[k] >> R) return fail(e, C2B_E_ARG, "c2b_annotate_build: listed slot out of range");
+        for (int r = 0; r < R; r++) {
+            const uint32_t m = meta[k * R + r];
+            if ((m >> 24) && ((int)(m & 0xffffu) > std::min(32 * NW, (int)C2B_MAX_ALN_LEN) || alns[k * R + r].n_edits > edit_cap))
+                return fail(e, C2B_E_ARG, "c2b_annotate_build: alignment wider than the op words, or an incomplete edit list");
+        }
+    }
+    if (chunk <= 0) chunk = 1 << 16;
+    // constant tables: names, labels, reference sequences, complement table
+    std::string tab;
+    std::vector<int32_t> name_off(1, 0), label_off(1, 0), ref_off(1, 0);
+    std::string nm, lb, rs;
+    for (int i = 0; i < n_names; i++) { nm += names[i]; name_off.push_back((int32_t)nm.size()); }
+    for (int i = 0; i < n_labels; i++) { lb += labels[i]; label_off.push_back((int32_t)lb.size()); }
+    for (int r = 0; r < R; r++) { rs.append(ref_seqs[r], (size_t)ref_lens[r]); ref_off.push_back((int32_t)rs.size()); }
+    auto al = [](size_t x) { return (x + 255) & ~(size_t)255; };
+    size_t t_names = 0, t_noff = al(nm.size()), t_rev = t_noff + al(name_off.size() * 4), t_lab = t_rev + al((size_t)n_names),
+           t_loff = t_lab + al(lb.size()), t_ref = t_loff + al(label_off.size() * 4), t_roff = t_ref + al(rs.size()),
+           t_comp = t_roff + al(ref_off.size() * 4), t_end = t_comp + 256;
+    tab.assign(t_end, '\0');
+    memcpy(&tab[t_names], nm.data(), nm.size()); memcpy(&tab[t_noff], name_off.data(), name_off.size() * 4);
+    memcpy(&tab[t_rev], name_rev, (size_t)n_names); memcpy(&tab[t_lab], lb.data(), lb.size());
+    memcpy(&tab[t_loff], label_off.data(), label_off.size() * 4); memcpy(&tab[t_ref], rs.data(), rs.size());
+    memcpy(&tab[t_roff], ref_off.data(), ref_off.size() * 4); memcpy(&tab[t_comp], comp256, 256);
+    DevBuf d_tab, d_in, d_len, d_out;
+    uint8_t *h_in = nullptr, *h_out = nullptr; size_t h_in_cap = 0, h_out_cap = 0;
+    auto cleanup = [&]() { rt_free(d_tab.p); rt_free(d_in.p); rt_free(d_len.p); rt_free(d_out.p); rt_host_free(h_in); rt_host_free(h_out); };
+    auto grow_host = [](uint8_t *&p, size_t &cap, size_t n) {
+        if (n <= cap) return true;
+        rt_host_free(p); cap = n + n / 4 + 4096; p = (uint8_t *)rt_host_alloc(cap);
+        return p != nullptr;
+    };
+    std::unique_ptr<c2b_annotation> A(new c2b_annotation());
+    A->n = n_unique;
+    A->ann_off.assign(1, 0); A->cig_off.assign(1, 0);
+    A->flag.resize((size_t)n_unique); A->mapq.resize((size_t)n_unique); A->first.resize((size_t)n_unique);
+    int rc = ensure(e, d_tab, t_end);
+    if (!rc) { rt_err r = rt_h2d(d_tab.p, tab.data(), t_end, e->stream); if (r != RT_OK) rc = fail(e, C2B_E_CUDA, "c2b_annotate_build: copy of the tables"); }
+    const size_t ER = (size_t)R, OW = (size_t)R * NW * 8, EW = (size_t)R * edit_cap * sizeof(c2b_edit);
+    auto one_chunk = [&](int64_t u0) -> int {
+        const int64_t u1 = std::min(n_unique, u0 + chunk), m = u1 - u0;
+        int64_t k0 = -1, k1 = 0;
+        for (int64_t u = u0; u < u1; u++) if (bidx[u] >= 0) { if (k0 < 0) k0 = bidx[u]; k1 = (int64_t)bidx[u] + 1; }
+        if (k0 < 0) k0 = k1 = 0;
+        const int64_t mk = k1 - k0;
+        const size_t rb = (size_t)(offsets[u1] - offsets[u0]);
+        // chunk input layout (device): reads | roff | bidx | recs | alns | ops | meta | edits | amask | aname | label
+        size_t o_reads = 0, o_roff = al(rb), o_bidx = o_roff + al((size_t)(m + 1) * 8), o_recs = o_bidx + al((size_t)m * 4),
+               o_alns = o_recs + al((size_t)mk * sizeof(c2b_read_rec)), o_ops = o_alns + al((size_t)mk * ER * sizeof(c2b_aln_rec)),
+               o_meta = o_ops + al((size_t)mk * OW), o_ed = o_meta + al((size_t)mk * ER * 4), o_am = o_ed + al((size_t)mk * EW),
+               o_an = o_am + al((size_t)mk * 4), o_lb = o_an + al((size_t)mk * 2), o_end = o_lb + al((size_t)mk * 4);
+        if (!grow_host(h_in, h_in_cap, o_end)) return fail(e, C2B_E_CUDA, "c2b_annotate_build: pinned allocation");
+        if (rb) memcpy(h_in + o_reads, reads + offsets[u0], rb);
+        int64_t *hro = (int64_t *)(h_in + o_roff);
+        for (int64_t u = 0; u <= m; u++) hro[u] = offsets[u0 + u] - offsets[u0];
+        int32_t *hb = (int32_t *)(h_in + o_bidx);
+        for (int64_t u = 0; u < m; u++) hb[u] = bidx[u0 + u] >= 0 ? (int32_t)(bidx[u0 + u] - k0) : -1;
+        if (mk) {
+            memcpy(h_in + o_recs, recs + k0, (size_t)mk * sizeof(c2b_read_rec));
+            memcpy(h_in + o_alns, alns + k0 * R, (size_t)mk * ER * sizeof(c2b_aln_rec));
+            memcpy(h_in + o_ops, ops + k0 * R * NW, (size_t)mk * OW);
+            memcpy(h_in + o_meta, meta + k0 * R, (size_t)mk * ER * 4);
+            if (EW) memcpy(h_in + o_ed, edits + k0 * R * edit_cap, (size_t)mk * EW);
+            memcpy(h_in + o_am, amask + k0, (size_t)mk * 4);
+            memcpy(h_in + o_an, aname + k0, (size_t)mk * 2);
+            memcpy(h_in + o_lb, label + k0, (size_t)mk * 4);
+        }
+        // lengths (2m) + offsets (2(m+1)) + flag / mapq / first
+        const size_t l_len = 0, l_aoff = al((size_t)2 * m * 8), l_coff = l_aoff + al((size_t)(m + 1) * 8),
+                     l_flag = l_coff + al((size_t)(m + 1) * 8), l_mapq = l_flag + al((size_t)m), l_first = l_mapq + al((size_t)m * 4),
+                     l_end = l_first + al((size_t)m * 2);
+        int rc2;
+        if ((rc2 = ensure(e, d_in, o_end)) || (rc2 = ensure(e, d_len, l_end))) return rc2;
+        RTCHK(rt_h2d(d_in.p, h_in, o_end, e->stream));
+        char *di = (char *)d_in.p, *dl = (char *)d_len.p, *dt = (char *)d_tab.p;
+        c2b::ann::AParams P;
+        memset(&P, 0, sizeof P);
+        P.reads = (const uint8_t *)(di + o_reads); P.roff = (const int64_t *)(di + o_roff); P.n = m;
+        P.bidx = (const int32_t *)(di + o_bidx); P.R = R; P.NW = NW; P.cap = edit_cap; P.flags = flags;
+        P.recs = (const c2b_read_rec *)(di + o_recs); P.alns = (const c2b_aln_rec *)(di + o_alns); P.ops = (const uint64_t *)(di + o_ops);
+        P.meta = (const uint32_t *)(di + o_meta); P.edits = (const c2b_edit *)(di + o_ed);
+        P.amask = (const uint32_t *)(di + o_am); P.aname = (const int16_t *)(di + o_an); P.label = (const int32_t *)(di + o_lb);
+        P.names = dt + t_names; P.name_off = (const int32_t *)(dt + t_noff); P.name_rev = (const uint8_t *)(dt + t_rev);
+        P.labels = dt + t_lab; P.label_off = (const int32_t *)(dt + t_loff);
+        P.refseq = dt + t_ref; P.ref_off = (const int32_t *)(dt + t_roff); P.comp = (const uint8_t *)(dt + t_comp);
+        P.ann_len = (int64_t *)(dl + l_len); P.cig_len = P.ann_len + m;
+        P.ann_off = (const int64_t *)(dl + l_aoff); P.cig_off = (const int64_t *)(dl + l_coff);
+        P.flag = (uint8_t *)(dl + l_flag); P.mapq = (int32_t *)(dl + l_mapq); P.first = (int16_t *)(dl + l_first);
+        int64_t tot[2] = {0, 0};
+#ifndef C2B_EMU
+        const int grid = (int)std::min<int64_t>((m + 7) / 8, 8192);
+        c2b_annotate_size_kernel<<<grid, 256, 0, e->stream>>>(P);
+        c2b_annotate_scan_kernel<<<1, 32, 0, e->stream>>>(P.ann_len, (int64_t *)P.ann_off, P.cig_len, (int64_t *)P.cig_off, m);
+        RTCHK(cudaGetLastError());
+        RTCHK(rt_d2h(&tot[0], P.ann_off + m, 8, e->stream));
+        RTCHK(rt_d2h(&tot[1], P.cig_off + m, 8, e->stream));
+        RTCHK(rt_sync(e->stream));
+#else
+        for (int64_t u = 0; u < m; u++) emu::run_warp([&]() { c2b::ann::annotate_one<false>(P, u); });
+        emu::run_warp([&]() { c2b::ann::scan_sizes(P.ann_len, (int64_t *)P.ann_off, m); c2b::ann::scan_sizes(P.cig_len, (int64_t *)P.cig_off, m); });
+        tot[0] = P.ann_off[m]; tot[1] = P.cig_off[m];
+#endif
+        if ((rc2 = ensure(e, d_out, (size_t)(tot[0] + tot[1]) + 16))) return rc2;
+        P.ann = (char *)d_out.p; P.cig = (char *)d_out.p + tot[0];
+#ifndef C2B_EMU
+        c2b_annotate_write_kernel<<<grid, 256, 0, e->stream>>>(P);
+        RTCHK(cudaGetLastError());
+#else
+        for (int64_t u = 0; u < m; u++) emu::run_warp([&]() { c2b::ann::annotate_one<true>(P, u); });
+#endif
+        const size_t l_tail = l_end - l_aoff, bytes = (size_t)(tot[0] + tot[1]);
+        if (!grow_host(h_out, h_out_cap, l_tail + bytes)) return fail(e, C2B_E_CUDA, "c2b_annotate_build: pinned allocation");
+        RTCHK(rt_d2h(h_out, dl + l_aoff, l_tail, e->stream));
+        RTCHK(rt_d2h(h_out + l_tail, d_out.p, bytes, e->stream));
+        RTCHK(rt_sync(e->stream));
+        const int64_t *ao = (const int64_t *)(h_out + 0), *co = (const int64_t *)(h_out + (l_coff - l_aoff));
+        const int64_t abase = A->ann_off.back(), cbase = A->cig_off.back();
+        for (int64_t u = 1; u <= m; u++) { A->ann_off.push_back(abase + ao[u]); A->cig_off.push_back(cbase + co[u]); }
+        A->ann.resize((size_t)(abase + tot[0])); A->cig.resize((size_t)(cbase + tot[1]));
+        if (tot[0]) memcpy(A->ann.data() + abase, h_out + l_tail, (size_t)tot[0]);
+        if (tot[1]) memcpy(A->cig.data() + cbase, h_out + l_tail + tot[0], (size_t)tot[1]);
+        memcpy(A->flag.data() + u0, h_out + (l_flag - l_aoff), (size_t)m);
+        memcpy(A->mapq.data() + u0, h_out + (l_mapq - l_aoff), (size_t)m * 4);
+        memcpy(A->first.data() + u0, h_out + (l_first - l_aoff), (size_t)m * 2);
+        return C2B_OK;
+    };
+    for (int64_t u0 = 0; !rc && u0 < n_unique; u0 += chunk) rc = one_chunk(u0);
+    cleanup();
+    if (rc) return rc;
+    *out = A.release();
+    return C2B_OK;
+}
+
+void c2b_annotate_free(c2b_annotation *a) { delete a; }
+int64_t c2b_annotate_n(const c2b_annotation *a) { return a ? a->n : 0; }
+const uint8_t *c2b_annotate_arena(const c2b_annotation *a) { return a ? a->ann.data() : nullptr; }
+const int64_t *c2b_annotate_offsets(const c2b_annotation *a) { return a ? a->ann_off.data() : nullptr; }
+const uint8_t *c2b_annotate_cigar_arena(const c2b_annotation *a) { return a ? a->cig.data() : nullptr; }
+const int64_t *c2b_annotate_cigar_offsets(const c2b_annotation *a) { return a ? a->cig_off.data() : nullptr; }
+const uint8_t *c2b_annotate_flags(const c2b_annotation *a) { return a ? a->flag.data() : nullptr; }
+const int32_t *c2b_annotate_mapq(const c2b_annotation *a) { return a ? a->mapq.data() : nullptr; }
+const int16_t *c2b_annotate_first(const c2b_annotation *a) { return a ? a->first.data() : nullptr; }
+const int64_t *c2b_annotate_last_record(const c2b_annotation *a) { return a && !a->last_rec.empty() ? a->last_rec.data() : nullptr; }
+const uint8_t *c2b_annotate_record_arena(const c2b_annotation *a) { return a ? (const uint8_t *)a->rec.data() : nullptr; }
+const int64_t *c2b_annotate_record_offsets(const c2b_annotation *a) { return a && !a->rec_off.empty() ? a->rec_off.data() : nullptr; }
 
 // pinned host memory for callers that want full-speed copies (bench.py, the Python wrapper)
 void *c2b_host_alloc(size_t n)

@@ -851,3 +851,246 @@ extern "C" int c2b_serial_stats(const c2b_read_rec *recs, const c2b_aln_rec *aln
     }
     return C2B_OK;
 }
+
+// ------------------------------------------------------------------------------------------------ annotated output
+// Replaces the record loops of process_fastq_write_out (CRISPRessoCORE.py:2293-2346) and process_single_fastq_write_bam_out
+// (:2387-2502): the input FASTQ is read again, split into records by the text-mode readline() rules of the ingest (universal
+// newlines; a record starts at every line and takes the next three, present or not), each record's sequence found in a hash of
+// the unique reads (byte compare), and the record written with its read's annotation (c2b_annotation, built on the device).
+namespace {
+
+struct TLine { size_t p; uint32_t len; };
+
+// lines under universal newlines ("\n", "\r\n", lone "\r"), indexed by all host threads from cuts placed right after a terminator
+void split_text_lines(const uint8_t *data, size_t n, std::vector<TLine> &lines)
+{
+    const int T = host_threads(n);
+    std::vector<size_t> cut((size_t)T + 1, 0);
+    cut[(size_t)T] = n;
+    for (int t = 1; t < T; t++) {
+        size_t p = std::max(cut[(size_t)t - 1], n / (size_t)T * (size_t)t);
+        while (p < n && data[p] != '\n' && data[p] != '\r') p++;
+        if (p < n) p += (data[p] == '\r' && p + 1 < n && data[p + 1] == '\n') ? 2 : 1;
+        cut[(size_t)t] = std::min(p, n);
+    }
+    std::vector<std::vector<TLine>> part((size_t)T);
+    run_threads(T, [&](int t) {
+        std::vector<TLine> &L = part[(size_t)t];
+        size_t p = cut[(size_t)t];
+        const size_t e = cut[(size_t)t + 1];
+        L.reserve((e - p) / 60 + 16);
+        while (p < e) {
+            size_t q = p;
+            while (q < e && data[q] != '\n' && data[q] != '\r') q++;
+            L.push_back({p, (uint32_t)(q - p)});
+            p = q < e ? q + ((data[q] == '\r' && q + 1 < e && data[q + 1] == '\n') ? 2 : 1) : e;
+        }
+    });
+    size_t tot = 0;
+    for (auto &L : part) tot += L.size();
+    lines.clear();
+    lines.reserve(tot);
+    for (auto &L : part) lines.insert(lines.end(), L.begin(), L.end());
+}
+
+struct UniqueIndex {                                         // exact sequence -> unique read index
+    const uint8_t *seqs; const int64_t *off; std::vector<int64_t> slot; uint64_t mask = 0;
+    UniqueIndex(const uint8_t *s, const int64_t *o, int64_t n) : seqs(s), off(o)
+    {
+        size_t cap = 16;
+        while (cap < (size_t)n * 2) cap <<= 1;
+        slot.assign(cap, -1); mask = cap - 1;
+        for (int64_t u = 0; u < n; u++) {
+            uint64_t h = hash_bytes(s + o[u], (size_t)(o[u + 1] - o[u])) & mask;
+            while (slot[h] >= 0) h = (h + 1) & mask;
+            slot[h] = u;
+        }
+    }
+    int64_t find(const uint8_t *p, size_t len) const
+    {
+        uint64_t h = hash_bytes(p, len) & mask;
+        for (; slot[h] >= 0; h = (h + 1) & mask) {
+            const int64_t u = slot[h];
+            if ((size_t)(off[u + 1] - off[u]) == len && (len == 0 || memcmp(seqs + off[u], p, len) == 0)) return u;
+        }
+        return -1;
+    }
+};
+
+struct TextInput {
+    c2b_bytes buf;
+    std::vector<TLine> lines;
+    bool last_open = false;                                  // the last line has no terminator
+    std::string err;
+    bool load(const char *path)
+    {
+        const size_t L = strlen(path);
+        const bool gz = L > 3 && strcmp(path + L - 3, ".gz") == 0;          // CRISPRessoCORE.py:2288, :2380
+        if (!(gz ? read_gz(path, buf, err) : read_plain(path, buf, err))) return false;
+        const size_t n = buf.size();
+        std::atomic<bool> wide(false);
+        const int T = host_threads(n);
+        run_threads(T, [&](int t) {
+            const size_t a = n * (size_t)t / T, b = n * (size_t)(t + 1) / T;
+            for (size_t i = a; i < b; i++) if (buf[i] & 0x80) { wide.store(true); return; }
+        });
+        if (wide.load()) { err = "non-ASCII byte in the FASTQ input (out of contract for the annotated outputs)"; return false; }
+        split_text_lines(buf.data(), n, lines);
+        last_open = n && buf[n - 1] != '\n' && buf[n - 1] != '\r';
+        return true;
+    }
+    bool has(size_t k) const { return k < lines.size(); }
+    bool ends(size_t k) const { return k + 1 < lines.size() || !last_open; }
+    Seq stripped(size_t k) const
+    {
+        Seq s{buf.data(), 0};
+        if (!has(k)) return s;
+        s.p = buf.data() + lines[k].p; s.len = lines[k].len;
+        while (s.len && is_space(s.p[0])) { s.p++; s.len--; }
+        while (s.len && is_space(s.p[s.len - 1])) s.len--;
+        return s;
+    }
+};
+
+}  // namespace
+
+// FASTQ: id + seq + "\n" + plus + annotation + "\n" + qual per record (id and quality keep their newline), gzip, one member per
+// thread and per 32 MB of text (a multi-member file whose decompressed bytes are what gzip.open(.., 'wt') would have written)
+extern "C" int c2b_annotate_write_fastq(const c2b_annotation *a, const uint8_t *seqs, const int64_t *offsets, int64_t n_unique,
+                                        const char *in_path, const char *out_path, int32_t n_threads)
+{
+    if (!a || !in_path || !out_path || n_unique != a->n || (n_unique && !offsets)) { g_fastq_err = "c2b_annotate_write_fastq: bad argument"; return C2B_E_ARG; }
+    TextInput in;
+    if (!in.load(in_path)) { g_fastq_err = "c2b_annotate_write_fastq: " + in.err; return C2B_E_ARG; }
+    const UniqueIndex idx(seqs, offsets, n_unique);
+    const int64_t n_rec = (int64_t)((in.lines.size() + 3) / 4);
+    int T = n_threads > 0 ? n_threads : (int)std::thread::hardware_concurrency();
+    T = std::max(1, std::min(T, 64));
+    if (n_rec < 4096) T = 1;
+    std::vector<std::string> outs((size_t)T);
+    std::vector<int> bad((size_t)T, 0);
+    const uint8_t *D = in.buf.data();
+    run_threads(T, [&](int t) {
+        const int64_t lo = n_rec * t / T, hi = n_rec * (t + 1) / T;
+        std::string o, z;
+        o.reserve(40 << 20);
+        auto flush = [&]() {
+            if (!gz_member(o, z)) return false;
+            outs[(size_t)t] += z; o.clear();
+            return true;
+        };
+        for (int64_t r = lo; r < hi; r++) {
+            const size_t k = (size_t)(4 * r);
+            const Seq sq = in.stripped(k + 1), pl = in.stripped(k + 2);
+            const int64_t u = idx.find(sq.p, sq.len);
+            if (u < 0) { bad[(size_t)t] = 1; return; }
+            o.append((const char *)D + in.lines[k].p, in.lines[k].len);
+            if (in.ends(k)) o.push_back('\n');
+            o.append((const char *)sq.p, sq.len); o.push_back('\n');
+            o.append((const char *)pl.p, pl.len);
+            o.append((const char *)a->ann.data() + a->ann_off[(size_t)u], (size_t)(a->ann_off[(size_t)u + 1] - a->ann_off[(size_t)u]));
+            o.push_back('\n');
+            if (in.has(k + 3)) { o.append((const char *)D + in.lines[k + 3].p, in.lines[k + 3].len); if (in.ends(k + 3)) o.push_back('\n'); }
+            if (o.size() >= (32u << 20) && !flush()) { bad[(size_t)t] = 2; return; }
+        }
+        if (!o.empty() && !flush()) bad[(size_t)t] = 2;
+    });
+    for (int b : bad) if (b) {
+        g_fastq_err = b == 1 ? "c2b_annotate_write_fastq: a read sequence is in neither variantCache nor the not-aligned reads" : "c2b_annotate_write_fastq: deflate failed";
+        return b == 1 ? C2B_E_ARG : C2B_E_STATE;
+    }
+    std::string tail;
+    bool any = false;
+    for (auto &s : outs) any |= !s.empty();
+    if (!any) { std::string e2; gz_member(e2, tail); }                 // an empty but valid gzip file
+    if (!write_parts(out_path, outs, tail)) { g_fastq_err = std::string("c2b_annotate_write_fastq: cannot write ") + out_path; return C2B_E_STATE; }
+    return C2B_OK;
+}
+
+// SAM: the header, then one line per record until the first record whose stripped id line is at most one character (the loop
+// condition of :2392); unaligned reads as flag 4, aligned ones at the first aligned reference's chr / start with its CIGAR, flag,
+// MAPQ, and reverse-complemented sequence / reversed quality when that reference's aln_strand is '-' (:2462-2469).  Records the
+// id and quality of each unique read's last record in the handle (sam_entry of :2497).
+extern "C" int c2b_annotate_write_sam(c2b_annotation *a, const uint8_t *seqs, const int64_t *offsets, int64_t n_unique,
+                                      const char *in_path, const char *sam_path, const char *header, int32_t n_names,
+                                      const char *const *chr, const char *const *pos, const uint8_t *rev, int32_t n_threads)
+{
+    if (!a || !in_path || !sam_path || !header || n_unique != a->n || (n_unique && !offsets) || n_names < 0 ||
+        (n_names && (!chr || !pos || !rev))) { g_fastq_err = "c2b_annotate_write_sam: bad argument"; return C2B_E_ARG; }
+    TextInput in;
+    if (!in.load(in_path)) { g_fastq_err = "c2b_annotate_write_sam: " + in.err; return C2B_E_ARG; }
+    const UniqueIndex idx(seqs, offsets, n_unique);
+    int64_t n_rec = 0;
+    while (in.has((size_t)(4 * n_rec)) && in.stripped((size_t)(4 * n_rec)).len > 1) n_rec++;
+    int T = n_threads > 0 ? n_threads : (int)std::thread::hardware_concurrency();
+    T = std::max(1, std::min(T, 64));
+    if (n_rec < 4096) T = 1;
+    std::vector<std::string> outs((size_t)T + 1);
+    outs[0] = header;
+    std::vector<int64_t> rec_u((size_t)n_rec, -1);
+    std::vector<int> bad((size_t)T, 0);
+    unsigned char comp[256];
+    for (int c = 0; c < 256; c++) comp[c] = 0;
+    comp['A'] = 'T'; comp['C'] = 'G'; comp['G'] = 'C'; comp['T'] = 'A'; comp['N'] = 'N'; comp['_'] = '_'; comp['-'] = '-';
+    run_threads(T, [&](int t) {
+        const int64_t lo = n_rec * t / T, hi = n_rec * (t + 1) / T;
+        std::string &o = outs[(size_t)t + 1];
+        std::string s2, q2;
+        for (int64_t r = lo; r < hi; r++) {
+            const size_t k = (size_t)(4 * r);
+            const Seq id = in.stripped(k), sq = in.stripped(k + 1), ql = in.stripped(k + 3);
+            const int64_t u = idx.find(sq.p, sq.len);
+            if (u < 0) { bad[(size_t)t] = 1; return; }
+            rec_u[(size_t)r] = u;
+            const uint8_t fl = a->flag[(size_t)u];
+            const int f = a->first[(size_t)u];
+            if (fl != 255 && (f < 0 || f >= n_names)) { bad[(size_t)t] = 2; return; }
+            o.append((const char *)id.p + 1, id.len - 1);
+            const char *sp = (const char *)sq.p, *qp = (const char *)ql.p;
+            if (fl == 255) o += "\t4\t*\t0\t0\t*\t*\t0\t0\t";
+            else {
+                o.push_back('\t'); o += std::to_string((int)fl); o.push_back('\t'); o += chr[f]; o.push_back('\t'); o += pos[f];
+                o.push_back('\t'); o += std::to_string(a->mapq[(size_t)u]); o.push_back('\t');
+                o.append((const char *)a->cig.data() + a->cig_off[(size_t)u], (size_t)(a->cig_off[(size_t)u + 1] - a->cig_off[(size_t)u]));
+                o += "\t*\t0\t0\t";
+                if (rev[f]) {                                  // CRISPRessoShared.reverse_complement (:399-403), quality reversed
+                    s2.assign(sq.len, ' '); q2.assign(ql.len, ' ');
+                    for (uint32_t i = 0; i < sq.len; i++) {
+                        unsigned char c = sq.p[sq.len - 1 - i];
+                        if (c >= 'a' && c <= 'z') c = (unsigned char)(c - 32);
+                        if (!comp[c]) { bad[(size_t)t] = 3; return; }
+                        s2[i] = (char)comp[c];
+                    }
+                    for (uint32_t i = 0; i < ql.len; i++) q2[i] = (char)ql.p[ql.len - 1 - i];
+                    sp = s2.data(); qp = q2.data();
+                }
+            }
+            o.append(sp, sq.len); o.push_back('\t'); o.append(qp, ql.len);
+            o += "\tc2:Z:";
+            const int64_t a0 = a->ann_off[(size_t)u], a1 = a->ann_off[(size_t)u + 1];
+            if (a1 > a0) o.append((const char *)a->ann.data() + a0 + 1, (size_t)(a1 - a0 - 1));
+            o.push_back('\n');
+        }
+    });
+    for (int b : bad) if (b) {
+        g_fastq_err = b == 1 ? "c2b_annotate_write_sam: a read sequence is in neither variantCache nor the not-aligned reads"
+                    : b == 2 ? "c2b_annotate_write_sam: reference name id out of range" : "c2b_annotate_write_sam: symbol without a complement";
+        return C2B_E_ARG;
+    }
+    if (!write_parts(sam_path, outs, std::string())) { g_fastq_err = std::string("c2b_annotate_write_sam: cannot write ") + sam_path; return C2B_E_STATE; }
+    a->last_rec.assign((size_t)n_unique, -1);
+    for (int64_t r = 0; r < n_rec; r++) a->last_rec[(size_t)rec_u[(size_t)r]] = r;
+    a->rec.clear();
+    a->rec_off.assign(1, 0);
+    a->rec_off.reserve((size_t)n_unique * 2 + 1);
+    for (int64_t u = 0; u < n_unique; u++) {
+        const int64_t r = a->last_rec[(size_t)u];
+        if (r >= 0) {
+            const Seq id = in.stripped((size_t)(4 * r)), ql = in.stripped((size_t)(4 * r + 3));
+            a->rec.append((const char *)id.p + 1, id.len - 1); a->rec_off.push_back((int64_t)a->rec.size());
+            a->rec.append((const char *)ql.p, ql.len);
+        } else a->rec_off.push_back((int64_t)a->rec.size());
+        a->rec_off.push_back((int64_t)a->rec.size());
+    }
+    return C2B_OK;
+}

@@ -23,6 +23,23 @@ template <class T> struct c2b_noinit_alloc : std::allocator<T> {
 };
 using c2b_bytes = std::vector<uint8_t, c2b_noinit_alloc<uint8_t>>;
 
+// Read annotations of --fastq_output / --bam_output (built by c2b_annotate_build in c2b_engine.cu, written out by
+// c2b_annotate_write_fastq / _sam in c2b_fastq.cpp).  Per unique read u: annotation text ann[ann_off[u] .. ann_off[u+1]) (the
+// FASTQ form, with its leading space), CIGAR of the first aligned reference, SAM flag (255: not aligned), MAPQ, name id of the
+// first aligned reference.
+struct c2b_annotation {
+    int64_t n = 0;
+    c2b_bytes ann, cig;
+    std::vector<int64_t> ann_off, cig_off;
+    std::vector<uint8_t> flag;
+    std::vector<int32_t> mapq;
+    std::vector<int16_t> first;
+    // set by c2b_annotate_write_sam: id and quality of each unique read's last record (rec[rec_off[2u] .. rec_off[2u+1]) and
+    // rec[rec_off[2u+1] .. rec_off[2u+2])), last_rec[u] = -1 when no record of it was written
+    std::vector<int64_t> last_rec, rec_off;
+    std::string rec;
+};
+
 // whole file into memory (c2b_fastq.cpp): plain read / gzip inflate (blocked gzip: all host threads)
 bool c2b_fastq_read_gz(const char *path, c2b_bytes &buf, std::string &err);
 void c2b_fastq_set_error(const std::string &m);

@@ -7,6 +7,8 @@ also usable as CRISPRessoPooled / CRISPRessoBatch's `--crispresso_command "pytho
 What is re-bound (INTEGRATION.md section 2), nothing else of the reference changes:
   * CRISPRessoCORE.process_fastq (module global, resolved by name at CRISPRessoCORE.py:3750; also reached through
     process_fastq_write_out :2285 and process_single_fastq_write_bam_out :2373)   -> crispresso2_b200.core.process_fastq
+  * CRISPRessoCORE.process_fastq_write_out / process_single_fastq_write_bam_out (--fastq_output / --bam_output, :3739-3743)
+    -> crispresso2_b200.annotate (single process; under torchrun the reference's wrappers stay bound)
   * CRISPRessoCORE.process_paired_fastq (--crispresso_merge, :3744-3748)   -> crispresso2_b200.paired: the reference's loop with its
     global_align calls answered from one GPU batch over every distinct mate sequence
   * filterFastqs.filterFastqs (imported and called at CRISPRessoCORE.py:3716-3717)          -> crispresso2_b200.filter_fastqs.filterFastqs
@@ -67,6 +69,23 @@ def bind(CORE=None, engine=None, lib_path=None):
                   engine=get_engine(), aln_matrix=matrix)
 
     CORE.process_fastq = process_fastq
+    if world == 1:
+        # --fastq_output / --bam_output: annotations built on the GPU, records written natively (annotate.py).  Like the
+        # reference's wrappers (:2285, :2373) they call the module-global process_fastq as it is bound when they run.
+        from . import annotate
+
+        def process_fastq_write_out(fastq_input, fastq_output, variantCache, ref_names, refs, args, files_to_remove, output_directory):
+            return annotate.process_fastq_write_out(fastq_input, fastq_output, variantCache, ref_names, refs, args, files_to_remove,
+                                                    output_directory, process_fastq=CORE.process_fastq)
+
+        def process_single_fastq_write_bam_out(fastq_input, bam_output, bam_header, variantCache, ref_names, refs, args,
+                                               files_to_remove, output_directory):
+            return annotate.process_single_fastq_write_bam_out(fastq_input, bam_output, bam_header, variantCache, ref_names, refs,
+                                                               args, files_to_remove, output_directory,
+                                                               process_fastq=CORE.process_fastq)
+
+        CORE.process_fastq_write_out = process_fastq_write_out
+        CORE.process_single_fastq_write_bam_out = process_single_fastq_write_bam_out
     # paired-end merge mode (--crispresso_merge): the reference's own loop over one batch of GPU alignments (paired.py)
     from . import paired
     reference_paired = CORE.process_paired_fastq

@@ -26,17 +26,22 @@ class LazyVariant(dict):
     _src = None                                        # per-batch subclass attribute: the BatchSource
 
     # no Python-level __init__: instances are created half a million at a time (c2b_pyext.fill_cache); `_k` is the read's
-    # index in the batch until the entry is materialised, -1 (or unset) afterwards
+    # index k in the batch until the entry is materialised, -2 - k afterwards (-1: unset)
 
     # -- materialisation ---------------------------------------------------------------------------------------
     def _fill(self):
         k = getattr(self, "_k", -1)
         if k >= 0:
-            self._k = -1
+            self._k = -2 - k
             src = type(self)._src
             full = src.variant(k)
             full["count"] = dict.__getitem__(self, "count") if dict.__contains__(self, "count") else int(src.counts[k])
             dict.update(self, full)
+            src.n_filled += 1
+            for key, value_of in src.extra_keys:       # keys the annotated-output writers set (annotate.py): last, as there
+                v = value_of(k)
+                if v is not None:
+                    dict.__setitem__(self, key, v)
 
     def __missing__(self, key):
         k = getattr(self, "_k", -1)
@@ -154,6 +159,8 @@ class BatchSource:
         self.counts = counts                               # dedup multiplicity per read (variant['count'])
         self.parts = parts if parts is not None else [(0, res, fix or {})]
         self.starts = [p[0] for p in self.parts]
+        self.n_filled = 0                                  # entries materialised so far
+        self.extra_keys = []                               # [(key, value_of(k) -> value or None)], see LazyVariant._fill
 
     def variant(self, k):
         import bisect

@@ -368,6 +368,52 @@ int32_t c2b_alleles_cut_width(const c2b_alleles *a);
 int  c2b_alleles_cut_fetch(const c2b_alleles *a, uint8_t *seq, uint8_t *ref, int32_t *wlen, uint8_t *unedited, int32_t *n_deleted,
                            int32_t *n_inserted, int32_t *n_mutated, int64_t *reads, double *pct);
 
+/* ---- annotated outputs: --fastq_output / --bam_output (csrc/c2b_annotate.cuh on the device, writers in csrc/c2b_fastq.cpp) ----
+ * replaces: the per-read annotation of process_fastq_write_out (CRISPRessoCORE.py:2302-2343) and
+ * process_single_fastq_write_bam_out (:2399-2497): ALN / ALN_SCORES / ALN_DETAILS / CLASS / MODS / DEL / INS / SUB / ALN_REF /
+ * ALN_SEQ text per unique read, and the SAM CIGAR (CRISPRessoShared.CIGAR_LOOKUP + unexplode_cigar, CRISPRessoShared.py:426-434,
+ * 561-582), flag and MAPQ of its first aligned reference.  Unique read u (reads / offsets) is batch read bidx[u] of the compact
+ * outputs (recs / alns: [n][R], ops: [n][R][NW], meta: [n][R], edits: [n][R][edit_cap], complete lists), or -1 when it was
+ * not in the batch (outside the engine's contract: "ALN=NA" with no scores).  Per batch read, decided by the host:
+ * amask = slots listed in aln_ref_names (ascending; 0 = not aligned), aname = name id of the one listed slot when it is
+ * re-labelled (prime-editing scaffold), else -1, label = class_name id.  names[0..R) are the references' own names;
+ * name_rev[id] = refs[name]['aln_strand'] == '-'.  ref_seqs are the R amplicons as aligned.  Uniques go through the device in
+ * chunks of `chunk` (<= 0: 65536) through pinned buffers on the engine's stream. */
+typedef struct c2b_annotation c2b_annotation;
+int  c2b_annotate_build(c2b_engine *e, const uint8_t *reads, const int64_t *offsets, int64_t n_unique, const int32_t *bidx,
+                        int32_t R, int32_t NW, int32_t edit_cap, const c2b_read_rec *recs, const c2b_aln_rec *alns,
+                        const uint64_t *ops, const uint32_t *meta, const c2b_edit *edits,
+                        const uint32_t *amask, const int16_t *aname, const int32_t *label,
+                        int32_t n_names, const char *const *names, const uint8_t *name_rev,
+                        int32_t n_labels, const char *const *labels,
+                        const char *const *ref_seqs, const int32_t *ref_lens, const uint8_t *comp256, uint32_t flags,
+                        int64_t chunk, c2b_annotation **out);
+void c2b_annotate_free(c2b_annotation *a);
+int64_t        c2b_annotate_n(const c2b_annotation *a);
+const uint8_t *c2b_annotate_arena(const c2b_annotation *a);          /* annotation u: arena[offsets[u] .. offsets[u+1]), leading space */
+const int64_t *c2b_annotate_offsets(const c2b_annotation *a);        /* n + 1 */
+const uint8_t *c2b_annotate_cigar_arena(const c2b_annotation *a);
+const int64_t *c2b_annotate_cigar_offsets(const c2b_annotation *a);
+const uint8_t *c2b_annotate_flags(const c2b_annotation *a);          /* SAM flag, 255 = not aligned */
+const int32_t *c2b_annotate_mapq(const c2b_annotation *a);
+const int16_t *c2b_annotate_first(const c2b_annotation *a);          /* name id of the first aligned reference, -1 */
+/* after c2b_annotate_write_sam: record index of each unique read's last SAM line (-1: none), and its id / quality at
+ * arena[off[2u] .. off[2u+1]) / arena[off[2u+1] .. off[2u+2]) */
+const int64_t *c2b_annotate_last_record(const c2b_annotation *a);
+const uint8_t *c2b_annotate_record_arena(const c2b_annotation *a);
+const int64_t *c2b_annotate_record_offsets(const c2b_annotation *a);
+/* replaces: the record loop of process_fastq_write_out (:2293-2346).  The input is read again (plain, gzip, blocked gzip),
+ * split by text-mode readline() rules, every record matched to its unique read (seqs / offsets, the handle's order) by exact
+ * sequence; out_path is gzip, one member per thread and 32 MB of text.  C2B_E_ARG: non-ASCII input or a sequence that is in
+ * no table.  Host threads (n_threads <= 0: all). */
+int  c2b_annotate_write_fastq(const c2b_annotation *a, const uint8_t *seqs, const int64_t *offsets, int64_t n_unique,
+                              const char *in_path, const char *out_path, int32_t n_threads);
+/* replaces: the record loop of process_single_fastq_write_bam_out (:2387-2502) up to the samtools call: header, then one
+ * SAM line per record; chr / pos / rev per name id = refs[name]['aln_chr'], str(refs[name]['aln_start']), aln_strand == '-'. */
+int  c2b_annotate_write_sam(c2b_annotation *a, const uint8_t *seqs, const int64_t *offsets, int64_t n_unique,
+                            const char *in_path, const char *sam_path, const char *header, int32_t n_names,
+                            const char *const *chr, const char *const *pos, const uint8_t *rev, int32_t n_threads);
+
 /* replaces: filterFastqs.filterFastqs for paired input (CRISPResso2/filterFastqs.py:230-407, the seven run_*_pair variants): both
  * files in lockstep, a pair kept iff both mates pass; mate 2 strictly above the threshold when only the min or only the mean
  * filter is set (:262, :284); same error mapping as c2b_fastq_filter.                                              */

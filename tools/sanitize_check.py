@@ -68,3 +68,20 @@ eng.configure(w3.refs, w3.ref_names, m, -20, -2, 5, 2, w3.flags, 'ACGTN', 8)
 eng.counts_reset()
 res = eng.align_packed(w3.buf, w3.off, compact=True)
 print('hdr3', eng.path_counts(), eng.ring_counts(), int((res.recs['best_score_milli'] > 0).sum()))
+# read annotations of --fastq_output / --bam_output: size / scan / write kernels over HDR compact results, several chunks
+import tempfile, types
+from crispresso2_b200 import annotate, core
+d = tempfile.mkdtemp(prefix='c2b_sanitize_')
+fq = os.path.join(d, 'hdr.fastq')
+synth.write_fastq_fast(fq, w3.buf.reshape(w3.n, -1))
+a = types.SimpleNamespace(**vars(w3.params))
+a.use_legacy_insertion_quantification = False
+a.prime_editing_pegRNA_scaffold_seq = a.prime_editing_pegRNA_extension_seq = ''
+a.needleman_wunsch_aln_matrix_loc = 'EDNAFULL'
+a.n_processes = '1'
+cache = {}
+core.process_fastq(fq, cache, w3.ref_names, w3.refs, a, [], d, engine=eng, aln_matrix=m)
+A = annotate.Annotation(cache, w3.refs, chunk=700)
+A.write_fastq(fq, os.path.join(d, 'out.fastq.gz'))
+print('annotate', A.n, int(A.ann_off[-1]))
+import shutil; shutil.rmtree(d, ignore_errors=True)
