@@ -125,6 +125,10 @@ struct RefDev {
     const uint32_t *g42;           // [Ipad]         4*gi[row]   in both halves
     // ring-banded path (four pairs per warp): score bound of any alignment that leaves the band, see ring_bound()
     int32_t rg_ok, rg_smax, rg_gmax, rg_gsum;
+    // diagonal tier (c2b_diag_kernel, DESIGN.md section 3): a read with J == I whose ungapped score beats dg_thr4 and the exact
+    // edge-run scores of the offsets 1..dg_S on either side is aligned on the main diagonal, no DP needed
+    int32_t dg_ok, dg_S, dg_thr4;
+    int32_t dg_c4[2 * 4 + 1];      // [s + 4]: 4 x (gap costs + incentives) of the path on offset diagonal s (edge runs only)
 };
 
 struct KParams {
@@ -150,9 +154,11 @@ struct KParams {
     uint64_t *gops; uint32_t *gmeta; int32_t NW;            // NW = W / 32 words of 32 ops per slot
     int32_t *left; unsigned long long *left_n;              // ALIGN kernel: pairs left over for the general kernel, and their count
     int32_t *left2; unsigned long long *left2_n;            // ALIGN kernel, narrow first tier: reads for the second-tier launch (nullptr: no narrow tier)
+    int32_t *left0; unsigned long long *left0_n;            // diagonal tier: reads it did not prove, for the narrow tier, and their count
+    unsigned long long *diag_n;                             // diagonal tier: [0] reads proved, [1] reads put on its list (cumulative)
     const unsigned long long *n_dev;                        // general kernel over the left-over list: *n_dev reads (entries of pair_order)
     int32_t discard_slab;                                   // ALIGN kernel: drop the dead slab lines from L2 instead of writing them back
-    unsigned long long *stats;             // cumulative path statistics (c2b_path_counts), indices 2..6
+    unsigned long long *stats;             // cumulative path statistics (c2b_path_counts), indices 2..7; [26] reads sent to the second tier
     int32_t vstride, hstride;
     const uint32_t *stage_src;        // = refs[0].prof2 (global source of the staged tile)
     int32_t stage_bytes;              // bytes of refs[0].prof2 staged into shared memory by TMA at kernel start (0: none)

@@ -247,9 +247,19 @@ __global__ void __launch_bounds__(WARPS_PER_CTA * 32, C2B_A_MIN_CTAS) c2b_align_
             if (w >= total) break;
             if (w + ahead < total) {                            // the unit this warp is likely to get next: bytes towards L2
                 const int64_t g = (int64_t)w + ahead;
-                const int64_t last = 16 * g + 16 < nrd ? 16 * g + 16 : nrd;
-                const int64_t a = P.offsets[16 * g] + (int64_t)(threadIdx.x & 31) * 128;
-                if (a < P.offsets[last]) asm volatile("prefetch.global.L2 [%0];" ::"l"(P.reads + a));
+                if (!P.pair_order) {
+                    const int64_t last = 16 * g + 16 < nrd ? 16 * g + 16 : nrd;
+                    const int64_t a = P.offsets[16 * g] + (int64_t)(threadIdx.x & 31) * 128;
+                    if (a < P.offsets[last]) asm volatile("prefetch.global.L2 [%0];" ::"l"(P.reads + a));
+                } else {                                        // reads of the diagonal tier's list: two lanes per read
+                    const int64_t x = 16 * g + ((threadIdx.x & 31) >> 1);
+                    if (x < nrd) {
+                        const int64_t rd = read_at(P, x);
+                        const int64_t b1 = P.offsets[rd + 1];
+                        for (int64_t a = (P.offsets[rd] & ~(int64_t)127) + (int64_t)(threadIdx.x & 1) * 128; a < b1; a += 256)
+                            asm volatile("prefetch.global.L2 [%0];" ::"l"(P.reads + a));
+                    }
+                }
             }
             if (!align_narrow16(P, *S, staged_prof, (int64_t)w, warp_slot)) {
                 align_group(P, *S, staged_prof, 2 * (int64_t)w, warp_slot);
@@ -275,6 +285,23 @@ __global__ void __launch_bounds__(WARPS_PER_CTA * 32, C2B_A_MIN_CTAS) c2b_align_
         align_group(P, *S, staged_prof, (int64_t)w, warp_slot);
         __syncwarp();
     }
+}
+
+// Diagonal tier (c2b_split.cuh: diag_unit): one read per warp, units of 32 consecutive reads strided over the grid.
+constexpr int D_WARPS_PER_CTA = 8;
+__global__ void __launch_bounds__(D_WARPS_PER_CTA * 32) c2b_diag_kernel(const __grid_constant__ KParams P)
+{
+    __shared__ DSmem smem[D_WARPS_PER_CTA];
+    DSmem &S = smem[threadIdx.x >> 5];
+    dsmem_init(P, S);
+    const int64_t units = (P.n_reads + 31) / 32;
+    int proved = 0, seen = 0;
+    for (int64_t u = (int64_t)blockIdx.x * D_WARPS_PER_CTA + (threadIdx.x >> 5); u < units; u += (int64_t)gridDim.x * D_WARPS_PER_CTA) {
+        proved += diag_unit(P, S, u);
+        seen += P.n_reads - 32 * u < 32 ? (int)(P.n_reads - 32 * u) : 32;
+        __syncwarp();
+    }
+    if ((threadIdx.x & 31) == 0 && seen) { wp::addg(P.diag_n, proved); wp::addg(P.diag_n + 1, seen - proved); }
 }
 
 // CLASSIFY kernel (c2b_split.cuh: classify_read): one aligned read per warp, reads strided over the grid.
@@ -333,14 +360,15 @@ struct c2b_engine {
     unsigned long long *d_counts = nullptr; size_t counts_n = 0;
     // scratch
     DevBuf tb, tbb, tbq, bnd, ops, rgo, work, lut;
-    DevBuf gops, gmeta, left, left2;   // device-pointer API: op streams / meta words / left-over list of the last launch
+    DevBuf gops, gmeta, left, left2, left0;   // device-pointer API: op streams / meta words / left-over lists of the last launch
     int n_warps = 0, grid = 0, wpc = 8, stage_cap = 0;
     int grid_a = 0, grid_b = 0, stage_cap_a = 0;       // ALIGN / CLASSIFY kernels
     int split_ok = 0, split_all = 0;                   // configuration admits the two-kernel form (some / all references)
+    int diag_any = 0;                                  // some reference admits the diagonal tier (RefDev::dg_ok)
     int numa_node = -1;                                // NUMA node of the device (-1: unknown / single node)
     int scratch_TS = 0;
     // staging for the host-pointer API: two buffer sets, copy-in / compute / copy-out streams
-    struct Stage { DevBuf reads, off, cnt, qw, rid, recs, alns, str, ed, maxlen, ord, gops, gmeta, left, left2; int32_t *h_ord = nullptr; size_t h_ord_cap = 0; int64_t *h_off = nullptr; size_t h_off_cap = 0;
+    struct Stage { DevBuf reads, off, cnt, qw, rid, recs, alns, str, ed, maxlen, ord, gops, gmeta, left, left2, left0; int32_t *h_ord = nullptr; size_t h_ord_cap = 0; int64_t *h_off = nullptr; size_t h_off_cap = 0;
                    // pinned bounce buffers for callers whose arrays are pageable (numpy): copies to / from them run on host
                    // threads while the other set's kernels and DMA are in flight
                    uint8_t *h_in = nullptr, *h_out = nullptr; size_t h_in_cap = 0, h_out_cap = 0;
@@ -505,10 +533,10 @@ int c2b_create(int device, c2b_engine **out)
 void c2b_destroy(c2b_engine *e)
 {
     if (!e) return;
-    DevBuf *bufs[] = {&e->tb, &e->tbb, &e->tbq, &e->bnd, &e->ops, &e->rgo, &e->work, &e->lut, &e->gops, &e->gmeta, &e->left, &e->left2};
+    DevBuf *bufs[] = {&e->tb, &e->tbb, &e->tbq, &e->bnd, &e->ops, &e->rgo, &e->work, &e->lut, &e->gops, &e->gmeta, &e->left, &e->left2, &e->left0};
     for (DevBuf *b : bufs) if (b->p) rt_free(b->p);
     for (auto &st : e->stage) {
-        DevBuf *sb[] = {&st.reads, &st.off, &st.cnt, &st.qw, &st.rid, &st.recs, &st.alns, &st.str, &st.ed, &st.maxlen, &st.ord, &st.gops, &st.gmeta, &st.left, &st.left2};
+        DevBuf *sb[] = {&st.reads, &st.off, &st.cnt, &st.qw, &st.rid, &st.recs, &st.alns, &st.str, &st.ed, &st.maxlen, &st.ord, &st.gops, &st.gmeta, &st.left, &st.left2, &st.left0};
         if (st.h_ord) rt_host_free(st.h_ord);
         for (DevBuf *b : sb) if (b->p) rt_free(b->p);
         if (st.h_off) rt_host_free(st.h_off);
@@ -676,6 +704,31 @@ int c2b_configure(c2b_engine *e, const c2b_params *p, int32_t n_refs, const c2b_
         cum[0] = 0;
         for (int q = 0; q <= Ipad; q++) cum[q + 1] = (uint16_t)(cum[q] + (q < I && incl[q] ? 1 : 0));
         d.coding = rf.coding_mask != nullptr; d.tem = rf.tot_exon_len_mod; d.hist_zero = e->hist_zero;
+        {   // diagonal tier (c2b_diag_kernel): score bounds of every path other than the main diagonal, DESIGN.md section 3
+            const int64_t go = p->gap_open, ge = p->gap_extend, gi0 = rf.gap_incentive[0], gI = rf.gap_incentive[I];
+            int64_t gmin = gi0, gp = 0, smax = rf.score_rows[0];
+            for (int i = 0; i <= I; i++) { gmin = std::min(gmin, rf.gap_incentive[i]); gp = std::max(gp, rf.gap_incentive[i]); }
+            for (size_t k = 0; k < (size_t)p->nq * I; k++) smax = std::max(smax, rf.score_rows[k]);
+            // (b) an interior gap run (one gap_open): smax (I - g) + 2 g (ge + gp) + go - ge, largest at g = 1 when 2 (ge + gp) <= smax
+            int64_t thr = smax * (I - 1) + go + ge + 2 * gp;
+            // (c) a path through a border cell that holds the reference's min_score = gap_open * I * J
+            thr = std::max(thr, go * I * I + std::max<int64_t>(smax, 0) * I + 2 * (int64_t)I * gp);
+            // (a) offset diagonal t = |s| with its two edge runs: at most smax (I - t) + t (2 ge + gp) + gp, decreasing in t;
+            // offsets up to dg_S are scored exactly, the bound covers the rest
+            auto edge_bound = [&](int64_t t) { return smax * (I - t) + t * (2 * ge + gp) + gp; };
+            int S = 0;
+            while (S < 4 && S + 1 < I && edge_bound(S + 1) > thr) S++;
+            if (S + 1 < I) thr = std::max(thr, edge_bound(S + 1));
+            thr = std::max<int64_t>(thr, -(1ll << 28));
+            d.dg_ok = d.rg_ok && !d.coding && go <= ge && ge <= 0 && gmin >= 0 && 2 * (ge + gp) <= smax && I >= 2 && thr < (1ll << 28) &&
+                      !(p->flags & C2B_F_NO_RING);
+            d.dg_S = S; d.dg_thr4 = (int32_t)(4 * thr);
+            for (int s = -4; s <= 4; s++) {
+                const int64_t t = s < 0 ? -s : s;
+                d.dg_c4[s + 4] = (int32_t)(4 * (s == 0 ? 0 : 2 * ge * t + gi0 + (s > 0 ? rf.gap_incentive[I - std::min<int64_t>(t, I)] : t * gI)));
+            }
+            if (!d.dg_ok) { d.dg_S = 0; d.dg_thr4 = 0; }
+        }
         if (rf.coding_mask)
             for (int q = 0; q < I; q++) incl[q] |= (uint8_t)((rf.coding_mask[q] & 3) << 1);   // after cum[]: bit 0 stays the window
         cumx[0] = cums[0] = 0;
@@ -719,6 +772,8 @@ int c2b_configure(c2b_engine *e, const c2b_params *p, int32_t n_refs, const c2b_
         for (int r = 0; r < n_refs; r++) n_ok += (e->refdev[r].pk_maxJ > 0 && !e->refdev[r].coding) ? 1 : 0;     // the packed DP is admissible
         e->split_ok = !(p->flags & (C2B_F_NO_PAIRING | C2B_F_NO_RING)) && n_ok > 0;
         e->split_all = n_ok == n_refs;
+        e->diag_any = 0;
+        for (int r = 0; r < n_refs; r++) e->diag_any |= e->refdev[r].dg_ok ? 1 : 0;
     }
     e->scratch_TS = 0;
     e->configured = true;
@@ -738,8 +793,9 @@ int c2b_string_width(const c2b_engine *e, int32_t max_read_len)
     return (e->max_I + max_read_len + 31) & ~31;
 }
 
-// work block (u64): [2..6] cumulative path statistics; set s: [8 + 8 s] work hand-out counter, [9 + 8 s] widest alignment
-constexpr size_t WORK_BYTES = 24 * 8;
+// work block (u64): [2..7] cumulative path statistics, [24..26] the diagonal tier's (c2b_diag_counts); set s: [8 + 8 s] work
+// hand-out counter, [9 + 8 s] widest alignment, [15 + 8 s] length of the diagonal tier's list
+constexpr size_t WORK_BYTES = 32 * 8;
 
 static int ensure_scratch(c2b_engine *e, int maxJ)
 {
@@ -799,11 +855,13 @@ static int ensure_scratch(c2b_engine *e, int maxJ)
 // One batch on compute stream `cs` using scratch set `set` (0 or 1): the ALIGN / CLASSIFY pair followed by the general
 // kernel over what ALIGN left over -- or the general kernel alone where the two-kernel form does not apply.  Launches that
 // may overlap in time must use different sets; launches on the same stream are ordered.
-// d_gops / d_gmeta / d_left: op streams [n_reads * R * W/32] u64, meta words [n_reads * R], left-over list [n_reads + 8] i32.
+// d_gops / d_gmeta / d_left: op streams [n_reads * R * W/32] u64, meta words [n_reads * R], left-over list [n_reads + 8] i32;
+// d_left2 / d_left0: the narrow tier's and the diagonal tier's lists [n_reads + 16] i32 (nullptr: that tier is off).
 static int launch_on(c2b_engine *e, rt_stream cs, int set, const uint8_t *d_reads, const int64_t *d_offsets, int64_t n_reads,
                      int32_t max_read_len, const int32_t *d_count, const int32_t *d_qweight,
                      const int32_t *d_ref_id, c2b_read_rec *d_recs, c2b_aln_rec *d_alns,
-                     uint8_t *d_strings, c2b_edit *d_edits, uint64_t *d_gops, uint32_t *d_gmeta, int32_t *d_left, int32_t *d_left2 = nullptr)
+                     uint8_t *d_strings, c2b_edit *d_edits, uint64_t *d_gops, uint32_t *d_gmeta, int32_t *d_left, int32_t *d_left2 = nullptr,
+                     int32_t *d_left0 = nullptr)
 {
     if (!e || !e->configured) return fail(e, C2B_E_STATE, "c2b_align_batch: engine not configured");
     if (n_reads < 0 || !d_recs || !d_alns || (n_reads && (!d_reads || !d_offsets))) return fail(e, C2B_E_ARG, "c2b_align_batch: bad argument");
@@ -876,6 +934,18 @@ static int launch_on(c2b_engine *e, rt_stream cs, int set, const uint8_t *d_read
         // length, or unsorted -- then hardly any unit of sixteen qualifies), one candidate reference per read
         const bool narrow = d_left2 && !P.pair_order && (e->n_refs == 1 || d_ref_id != nullptr) && !getenv("C2B_NO_NARROW");
         if (narrow) { A.left2 = d_left2; A.left2_n = wk + 5; }
+        // diagonal tier ahead of the narrow one: reads it proves are done, the narrow tier works through the rest (wk[7] of them).
+        // A batch smaller than one narrow unit (16 reads) goes through the groups of eight anyway and keeps them whole.
+        const bool diag = narrow && d_left0 && e->diag_any && n_reads >= 16 && !getenv("C2B_NO_DIAG");
+        if (diag) {
+            KParams D = P;
+            D.left0 = d_left0; D.left0_n = wk + 7; D.diag_n = P.stats + 24;
+            const int64_t units = (n_reads + 31) / 32;
+            const int grid_d = (int)std::min<int64_t>((units + D_WARPS_PER_CTA - 1) / D_WARPS_PER_CTA, (int64_t)e->grid_a * 16);
+            c2b_diag_kernel<<<grid_d, D_WARPS_PER_CTA * 32, 0, cs>>>(D);
+            e->launches++;
+            A.pair_order = d_left0; A.n_dev = wk + 7;
+        }
         c2b_align_kernel<<<e->grid_a, e->wpc * 32, smem_a, cs>>>(A);
         if (narrow) {                                         // second tier: what the narrow band did not settle, eight reads per group
             KParams A2 = A;
@@ -909,12 +979,25 @@ static int launch_on(c2b_engine *e, rt_stream cs, int set, const uint8_t *d_read
             const bool narrow = d_left2 && !P.pair_order && (e->n_refs == 1 || d_ref_id != nullptr) && !getenv("C2B_NO_NARROW");
             if (narrow) {
                 A.left2 = d_left2; A.left2_n = wk + 5;
-                for (int64_t w = 0; 16 * w < n_reads; w++)
+                int64_t n1 = n_reads;
+                if (d_left0 && e->diag_any && n_reads >= 16 && !getenv("C2B_NO_DIAG")) {    // diagonal tier, then the narrow tier over its list
+                    KParams D = P;
+                    D.left0 = d_left0; D.left0_n = wk + 7; D.diag_n = P.stats + 24;
+                    static DSmem DS;
+                    for (int64_t u = 0; 32 * u < n_reads; u++)
+                        emu::run_warp([&]() {
+                            dsmem_init(D, DS);
+                            const int k = diag_unit(D, DS, u), m = n_reads - 32 * u < 32 ? (int)(n_reads - 32 * u) : 32;
+                            if (wp::lane() == 0) { wp::addg(D.diag_n, k); wp::addg(D.diag_n + 1, m - k); }
+                        });
+                    A.pair_order = d_left0; A.n_dev = wk + 7; n1 = (int64_t)wk[7];
+                }
+                for (int64_t w = 0; 16 * w < n1; w++)
                     emu::run_warp([&]() {
                         if (!align_narrow16(A, AS, nullptr, w, 0)) {
                             align_group(A, AS, nullptr, 2 * w, 0);
                             wp::sync();
-                            if (8 * (2 * w + 1) < n_reads) align_group(A, AS, nullptr, 2 * w + 1, 0);
+                            if (8 * (2 * w + 1) < n1) align_group(A, AS, nullptr, 2 * w + 1, 0);
                         }
                     });
                 KParams A2 = A;
@@ -957,13 +1040,14 @@ static int launch_on(c2b_engine *e, rt_stream cs, int set, const uint8_t *d_read
 }
 
 // op-stream buffers of the device-pointer API (engine-owned, sized for the batch)
-static int ensure_ops(c2b_engine *e, DevBuf &gops, DevBuf &gmeta, DevBuf &left, DevBuf &left2, int64_t n_reads, int nr, int W)
+static int ensure_ops(c2b_engine *e, DevBuf &gops, DevBuf &gmeta, DevBuf &left, DevBuf &left2, DevBuf &left0, int64_t n_reads, int nr, int W)
 {
     int rc;
     if ((rc = ensure(e, gops, (size_t)n_reads * nr * (W / 32) * 8))) return rc;
     if ((rc = ensure(e, gmeta, (size_t)n_reads * nr * 4))) return rc;
     if ((rc = ensure(e, left, (size_t)(n_reads + 8) * 4))) return rc;
     if ((rc = ensure(e, left2, (size_t)(n_reads + 16) * 4))) return rc;
+    if ((rc = ensure(e, left0, (size_t)(n_reads + 16) * 4))) return rc;
     return C2B_OK;
 }
 
@@ -978,10 +1062,11 @@ int c2b_align_batch_device(c2b_engine *e, const uint8_t *d_reads, const int64_t 
 #endif
     if (max_read_len < 1) max_read_len = 1;
     const int W = (e->max_I + max_read_len + 31) & ~31, nr = d_ref_id ? 1 : e->n_refs;
-    int rc = ensure_ops(e, e->gops, e->gmeta, e->left, e->left2, n_reads, nr, W);
+    int rc = ensure_ops(e, e->gops, e->gmeta, e->left, e->left2, e->left0, n_reads, nr, W);
     if (rc) return rc;
     return launch_on(e, e->stream, 0, d_reads, d_offsets, n_reads, max_read_len, d_count, d_qweight, d_ref_id, d_recs,
-                     d_alns, d_strings, d_edits, (uint64_t *)e->gops.p, (uint32_t *)e->gmeta.p, (int32_t *)e->left.p, (int32_t *)e->left2.p);
+                     d_alns, d_strings, d_edits, (uint64_t *)e->gops.p, (uint32_t *)e->gmeta.p, (int32_t *)e->left.p, (int32_t *)e->left2.p,
+                     (int32_t *)e->left0.p);
 }
 
 int c2b_ops_device(c2b_engine *e, void **d_ops, void **d_meta)
@@ -1039,6 +1124,18 @@ int c2b_path_counts(c2b_engine *e, int64_t *pair_items, int64_t *single_items)
                 (long long)v[6], (long long)v[7]);
     if (pair_items) *pair_items = v[2] + (v[7] + 1) / 2;
     if (single_items) *single_items = v[3];
+    return C2B_OK;
+}
+
+int c2b_diag_counts(c2b_engine *e, int64_t *proved, int64_t *tier1, int64_t *tier2)
+{
+    if (!e || !e->work.p) return fail(e, C2B_E_STATE, "c2b_diag_counts: nothing launched yet");
+    int64_t v[3] = {0, 0, 0};
+    RTCHK(rt_d2h(v, (unsigned long long *)e->work.p + 24, sizeof v, e->stream));
+    RTCHK(rt_sync(e->stream));
+    if (proved) *proved = v[0];
+    if (tier1) *tier1 = v[1];
+    if (tier2) *tier2 = v[2];
     return C2B_OK;
 }
 
@@ -1222,7 +1319,7 @@ static int align_batch_host(c2b_engine *e, const uint8_t *reads, const int64_t *
         if (count && (rc = ensure(e, st.cnt, (size_t)n * 4))) return rc;
         if (qweight && (rc = ensure(e, st.qw, (size_t)n * 4))) return rc;
         if (ref_id && (rc = ensure(e, st.rid, (size_t)n * 4))) return rc;
-        if ((rc = ensure_ops(e, st.gops, st.gmeta, st.left, st.left2, n, nr, W))) return rc;
+        if ((rc = ensure_ops(e, st.gops, st.gmeta, st.left, st.left2, st.left0, n, nr, W))) return rc;
         if (st.h_off_cap < (size_t)(n + 1)) {
             if (st.h_off) rt_host_free(st.h_off);
             st.h_off = (int64_t *)rt_host_alloc((size_t)(n + 1) * 8); st.h_off_cap = st.h_off ? (size_t)(n + 1) : 0;
@@ -1280,7 +1377,7 @@ static int align_batch_host(c2b_engine *e, const uint8_t *reads, const int64_t *
                        count ? (const int32_t *)st.cnt.p : nullptr, qweight ? (const int32_t *)st.qw.p : nullptr,
                        ref_id ? (const int32_t *)st.rid.p : nullptr, (c2b_read_rec *)st.recs.p,
                        (c2b_aln_rec *)st.alns.p, strings ? (uint8_t *)st.str.p : nullptr,
-                       cap ? (c2b_edit *)st.ed.p : nullptr, (uint64_t *)st.gops.p, (uint32_t *)st.gmeta.p, (int32_t *)st.left.p, (int32_t *)st.left2.p);
+                       cap ? (c2b_edit *)st.ed.p : nullptr, (uint64_t *)st.gops.p, (uint32_t *)st.gmeta.p, (int32_t *)st.left.p, (int32_t *)st.left2.p, (int32_t *)st.left0.p);
         e->pair_order = nullptr;
         if (rc) return rc;
         // keep this batch's "widest alignment" before the next launch sequence resets it

@@ -563,8 +563,109 @@ C2B_DEV bool align_narrow16(const KParams &P, ASmem &S, const uint32_t *staged_p
     if (lane == 0) {
         wp::addg(P.stats + 7, wp::popc(pass2));
         wp::addg(P.stats + 5, wp::popc(pass2));
+        wp::addg(P.stats + 26, 16 - wp::popc(pass2));        // reads sent to the second tier (c2b_diag_counts)
     }
     return true;
+}
+
+// ---------------------------------------------------------------------------------------- ALIGN, diagonal tier (tier 0)
+// A read as long as its amplicon whose ungapped score on the main diagonal beats every other path is aligned there, with no
+// DP: it scores strictly above RefDev::dg_thr4 (the bound on paths with an interior gap run, on offset diagonals past dg_S and
+// on paths through the reference's min_score borders) and strictly above the exact score of each offset diagonal 1..dg_S with
+// its two edge runs.  Then the diagonal is the unique optimum and the reference's traceback returns it (DESIGN.md section 3).
+// One read per warp, 32 consecutive reads per unit; the unit's unproved reads go, in order and with one atomic, on the tier-0
+// list (P.left0) that the narrow tier works through.
+struct DSmem {                                         // diagonal tier, per warp
+    uint8_t fw[RG_COMBO], rc[RG_COMBO];
+    uint8_t lut[256];
+    int64_t off[33];
+    int32_t ref[32];
+};
+
+// true if read rd is proved (op stream and meta word written); all lanes call with warp-uniform arguments
+C2B_DEV bool diag_read(const KParams &P, DSmem &S, int64_t rd, int64_t off, int J, int r)
+{
+    const int lane = wp::lane();
+    const RefDev &R = refdev(P, r);
+    const int I = R.I;
+    // the reads the narrow tier would take (one candidate reference, packed ring admissible), of the amplicon's length
+    if (!R.dg_ok || J != I || J > RG_COMBO || J + 32 > P.TS || J > R.pk_maxJ || I + J > PK_MAX_ALN) return false;
+    const bool bad = load_codes_a(P, S.lut, off, J, S.fw, S.rc);
+    wp::sync();
+    if (bad) return false;
+    const int mode = strand_mode(P, R, S.fw, J);
+    if (mode == 2) return false;                     // both strands: the DP decides which one
+    const uint8_t *c = mode == 1 ? S.rc : S.fw;
+    const int32_t *prof = R.prof;                    // [q][Ipad]: 4 x matrix[reference row][alphabet[q]]
+    const int Ipad = R.Ipad, dS = R.dg_S;
+    int acc[9];                                      // acc[s + 4]: 4 x ungapped score of read base k + s against reference row k
+#pragma unroll
+    for (int s = 0; s < 9; s++) acc[s] = 0;
+    for (int k = lane; k < I; k += 32) {
+        const int32_t *pk = prof + k;
+#pragma unroll
+        for (int s = -4; s <= 4; s++) {
+            const int j = k + s;
+            if ((s < 0 ? -s : s) <= dS && j >= 0 && j < J) acc[s + 4] += pk[(int)c[j] * Ipad];
+        }
+    }
+#pragma unroll
+    for (int s = 0; s < 9; s++)
+#pragma unroll
+        for (int d = 16; d >= 1; d >>= 1) acc[s] += wp::shfl_xor(acc[s], d);
+    bool proved = acc[4] > R.dg_thr4;
+#pragma unroll
+    for (int s = -4; s <= 4; s++)
+        if (s != 0 && (s < 0 ? -s : s) <= dS) proved = proved && acc[4] > acc[s + 4] + R.dg_c4[s + 4];
+    if (!proved) return false;
+    // what align_narrow16 writes for an all-M traceback of I columns: op words of 32 ops, OP_NONE (3) past the end
+    const int64_t slot = oslot(P, rd, r);
+    if (lane < 16 && lane < P.NW) {
+        const int rem = I - 32 * lane;
+        P.gops[slot * P.NW + lane] = rem >= 32 ? 0ull : rem <= 0 ? ~0ull : (~0ull << (2 * rem));
+    }
+    if (lane == 0) P.gmeta[slot] = gmeta_pack(I, mode == 1, GM_ALIGNED);
+    return true;
+}
+
+C2B_DEV void dsmem_init(const KParams &P, DSmem &S)
+{
+    for (int k = wp::lane(); k < 256; k += 32) S.lut[k] = P.lut[k];
+    wp::sync();
+}
+
+// reads 32u .. 32u+31: returns the number proved
+C2B_DEV int diag_unit(const KParams &P, DSmem &S, int64_t u)
+{
+    const int lane = wp::lane();
+    const int64_t first = 32 * u;
+    const int n = P.n_reads - first < 32 ? (int)(P.n_reads - first) : 32;
+    {
+        const int64_t rd = first + lane;
+        if (lane < n) { S.off[lane] = P.offsets[rd]; S.ref[lane] = P.ref_id ? P.ref_id[rd] : 0; }
+        if (lane == 0) S.off[n] = P.offsets[first + n];
+    }
+    wp::sync();
+#ifndef C2B_EMU
+    {                                                // the unit's bytes towards L2 (about 8 KB), one request per line
+        const int64_t b0 = S.off[0] & ~(int64_t)127, b1 = S.off[n];
+        for (int64_t a = b0 + (int64_t)lane * 128; a < b1; a += 32 * 128) asm volatile("prefetch.global.L2 [%0];" ::"l"(P.reads + a));
+    }
+#endif
+    uint32_t fail = 0;
+#pragma unroll 1
+    for (int x = 0; x < n; x++) {
+        const int64_t off = S.off[x];
+        if (!diag_read(P, S, first + x, off, (int)(S.off[x + 1] - off), S.ref[x])) fail |= 1u << x;
+        wp::sync();
+    }
+    if (fail) {                                      // warp-aggregated append: the unit's leftovers stay in read order
+        unsigned long long pos = 0;
+        if (lane == 0) pos = wp::fetch_add(P.left0_n, (unsigned long long)wp::popc(fail));
+        pos = (unsigned long long)(uint32_t)wp::shfl((int)(uint32_t)pos, 0) | ((unsigned long long)(uint32_t)wp::shfl((int)(uint32_t)(pos >> 32), 0) << 32);
+        if ((fail >> lane) & 1u) P.left0[pos + wp::popc(fail & ((1u << lane) - 1u))] = (int32_t)(first + lane);
+    }
+    return n - wp::popc(fail);
 }
 
 // ------------------------------------------------------------------------------------------------- CLASSIFY

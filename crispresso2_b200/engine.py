@@ -286,5 +286,12 @@ class Engine:
         self.L.c2b_ring_counts(self.h, C.byref(a), C.byref(b))
         return a.value, b.value
 
+    def diag_counts(self):
+        """(reads proved on the main diagonal, reads the diagonal tier handed to the narrow tier, reads the narrow tier sent
+        to the wide ring) since the last counts_reset"""
+        a, b, c = C.c_int64(0), C.c_int64(0), C.c_int64(0)
+        self._check(self.L.c2b_diag_counts(self.h, C.byref(a), C.byref(b), C.byref(c)), "c2b_diag_counts")
+        return a.value, b.value, c.value
+
     def launch_count(self):
         return int(self.L.c2b_launch_count(self.h))
