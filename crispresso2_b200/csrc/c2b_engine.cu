@@ -294,17 +294,21 @@ __global__ void __launch_bounds__(D_WARPS_PER_CTA * 32) c2b_diag_kernel(const __
     __shared__ DSmem smem[D_WARPS_PER_CTA];
     DSmem &S = smem[threadIdx.x >> 5];
     dsmem_init(P, S);
+    ScAcc<1> acc;
+    sc_init(acc);
     const int64_t units = (P.n_reads + 31) / 32;
     int proved = 0, seen = 0;
     for (int64_t u = (int64_t)blockIdx.x * D_WARPS_PER_CTA + (threadIdx.x >> 5); u < units; u += (int64_t)gridDim.x * D_WARPS_PER_CTA) {
-        proved += diag_unit(P, S, u);
+        proved += diag_unit(P, S, u, acc);
         seen += P.n_reads - 32 * u < 32 ? (int)(P.n_reads - 32 * u) : 32;
         __syncwarp();
     }
+    sc_flush(acc, P);
     if ((threadIdx.x & 31) == 0 && seen) { wp::addg(P.diag_n, proved); wp::addg(P.diag_n + 1, seen - proved); }
 }
 
-// CLASSIFY kernel (c2b_split.cuh: classify_read): one aligned read per warp, reads strided over the grid.
+// CLASSIFY kernel (c2b_split.cuh: classify_read): one aligned read per warp, reads strided over the grid -- every read, or
+// (after the diagonal tier, which classifies the reads it proves) the entries of its list: P.pair_order, *P.n_dev of them.
 template <bool ONE>
 __global__ void __launch_bounds__(B_WARPS_PER_CTA * 32, C2B_B_MIN_CTAS) c2b_classify_kernel(const __grid_constant__ KParams P)
 {
@@ -312,26 +316,33 @@ __global__ void __launch_bounds__(B_WARPS_PER_CTA * 32, C2B_B_MIN_CTAS) c2b_clas
     BSmem &S = smem[threadIdx.x >> 5];
     const int64_t nw = (int64_t)gridDim.x * B_WARPS_PER_CTA;
     const int64_t total_bytes = P.offsets[P.n_reads];
-    int64_t rd = (int64_t)blockIdx.x * B_WARPS_PER_CTA + (threadIdx.x >> 5);
-    if (rd >= P.n_reads) return;
+    const int64_t n = nreads(P);
+    int64_t x = (int64_t)blockIdx.x * B_WARPS_PER_CTA + (threadIdx.x >> 5);      // position in the read order
+    if (x >= n) return;
     ScAcc<ONE ? 1 : RG_MAX_REFS> acc;
     sc_init(acc);
-    // two-deep input pipeline: stage A of read rd + 2 nw and stage B of read rd + nw are in flight while read rd is classified
+    // two-deep input pipeline: stage A of position x + 2 nw and stage B of x + nw are in flight while x is classified; the
+    // read at x + 3 nw is looked up one iteration before its stage A needs it (a list entry, then its offsets: two round trips)
+    int32_t rd = (int32_t)read_at(P, x), rd1 = 0, rd2 = 0;
     BPreA a1 = classify_pre_a(P, rd);
     BPre pre = classify_pre_b<ONE>(P, rd, a1, total_bytes);
-    if (rd + nw < P.n_reads) a1 = classify_pre_a(P, rd + nw);
-    while (rd < P.n_reads) {
+    if (x + nw < n) { rd1 = (int32_t)read_at(P, x + nw); a1 = classify_pre_a(P, rd1); }
+    if (x + 2 * nw < n) rd2 = (int32_t)read_at(P, x + 2 * nw);
+    while (x < n) {
         const BPre cur = pre;
+        const int32_t rc = rd;
         if (cur.go) classify_stage<ONE>(cur, S);
         __syncwarp();
-        const int64_t nxt = rd + nw;
-        if (nxt < P.n_reads) {
-            pre = classify_pre_b<ONE>(P, nxt, a1, total_bytes);
-            if (nxt + nw < P.n_reads) a1 = classify_pre_a(P, nxt + nw);
+        const int64_t nxt = x + nw;
+        if (nxt < n) {
+            pre = classify_pre_b<ONE>(P, rd1, a1, total_bytes);
+            rd = rd1;
+            if (nxt + nw < n) { a1 = classify_pre_a(P, rd2); rd1 = rd2; }
+            if (nxt + 2 * nw < n) rd2 = (int32_t)read_at(P, nxt + 2 * nw);
         }
-        if (cur.go) classify_read<ONE>(P, rd, cur, S, acc);
+        if (cur.go) classify_read<ONE>(P, rc, cur, S, acc);
         __syncwarp();
-        rd = nxt;
+        x = nxt;
     }
     sc_flush(acc, P);
 }
@@ -947,6 +958,8 @@ static int launch_on(c2b_engine *e, rt_stream cs, int set, const uint8_t *d_read
             A.pair_order = d_left0; A.n_dev = wk + 7;
         }
         c2b_align_kernel<<<e->grid_a, e->wpc * 32, smem_a, cs>>>(A);
+        KParams B = P;                                        // CLASSIFY: every read in batch order, or the diagonal tier's list
+        B.pair_order = diag ? d_left0 : nullptr; B.n_dev = diag ? wk + 7 : nullptr;
         if (narrow) {                                         // second tier: what the narrow band did not settle, eight reads per group
             KParams A2 = A;
             A2.left2 = nullptr; A2.left2_n = nullptr;
@@ -954,8 +967,8 @@ static int launch_on(c2b_engine *e, rt_stream cs, int set, const uint8_t *d_read
             c2b_align_kernel<<<e->grid_a, e->wpc * 32, smem_a, cs>>>(A2);
             e->launches++;
         }
-        if (one) c2b_classify_kernel<true><<<e->grid_b, B_WARPS_PER_CTA * 32, 0, cs>>>(P);
-        else c2b_classify_kernel<false><<<e->grid_b, B_WARPS_PER_CTA * 32, 0, cs>>>(P);
+        if (one) c2b_classify_kernel<true><<<e->grid_b, B_WARPS_PER_CTA * 32, 0, cs>>>(B);
+        else c2b_classify_kernel<false><<<e->grid_b, B_WARPS_PER_CTA * 32, 0, cs>>>(B);
         // the general kernel over ALIGN's left-over pairs (free-running warps, no ring-banded attempt)
         P.pair_order = d_left; P.n_dev = wk + 3; P.work_counter = wk + 2; P.tbq = nullptr; P.rgops = nullptr;
         P.tbb = nullptr;                                      // these pairs left the ring band: the banded slab would only cost a second DP
@@ -977,9 +990,10 @@ static int launch_on(c2b_engine *e, rt_stream cs, int set, const uint8_t *d_read
             A.left = d_left; A.left_n = wk + 3;
             emu::run_warp([&]() { asmem_init(A, AS); });
             const bool narrow = d_left2 && !P.pair_order && (e->n_refs == 1 || d_ref_id != nullptr) && !getenv("C2B_NO_NARROW");
+            const int32_t *order = nullptr;                   // CLASSIFY's read order (nullptr: all reads)
+            int64_t n1 = n_reads;
             if (narrow) {
                 A.left2 = d_left2; A.left2_n = wk + 5;
-                int64_t n1 = n_reads;
                 if (d_left0 && e->diag_any && n_reads >= 16 && !getenv("C2B_NO_DIAG")) {    // diagonal tier, then the narrow tier over its list
                     KParams D = P;
                     D.left0 = d_left0; D.left0_n = wk + 7; D.diag_n = P.stats + 24;
@@ -987,10 +1001,12 @@ static int launch_on(c2b_engine *e, rt_stream cs, int set, const uint8_t *d_read
                     for (int64_t u = 0; 32 * u < n_reads; u++)
                         emu::run_warp([&]() {
                             dsmem_init(D, DS);
-                            const int k = diag_unit(D, DS, u), m = n_reads - 32 * u < 32 ? (int)(n_reads - 32 * u) : 32;
+                            ScAcc<1> acc; sc_init(acc);
+                            const int k = diag_unit(D, DS, u, acc), m = n_reads - 32 * u < 32 ? (int)(n_reads - 32 * u) : 32;
+                            sc_flush(acc, D);
                             if (wp::lane() == 0) { wp::addg(D.diag_n, k); wp::addg(D.diag_n + 1, m - k); }
                         });
-                    A.pair_order = d_left0; A.n_dev = wk + 7; n1 = (int64_t)wk[7];
+                    A.pair_order = d_left0; A.n_dev = wk + 7; n1 = (int64_t)wk[7]; order = d_left0;
                 }
                 for (int64_t w = 0; 16 * w < n1; w++)
                     emu::run_warp([&]() {
@@ -1008,7 +1024,8 @@ static int launch_on(c2b_engine *e, rt_stream cs, int set, const uint8_t *d_read
             for (int64_t w = 0; 8 * w < n_reads; w++) emu::run_warp([&]() { align_group(A, AS, nullptr, w, 0); });
             static BSmem BS;
             const int64_t total_bytes = d_offsets[n_reads];
-            for (int64_t rd = 0; rd < n_reads; rd++) {
+            for (int64_t x = 0; x < n1; x++) {
+                const int64_t rd = order ? order[x] : x;
                 if (one) emu::run_warp([&]() { ScAcc<1> acc; sc_init(acc); const BPreA a = classify_pre_a(P, rd); const BPre b = classify_pre_b<true>(P, rd, a, total_bytes);
                                                if (b.go) { classify_stage<true>(b, BS); wp::sync(); classify_read<true>(P, rd, b, BS, acc); } sc_flush(acc, P); });
                 else emu::run_warp([&]() { ScAcc<RG_MAX_REFS> acc; sc_init(acc); const BPreA a = classify_pre_a(P, rd); const BPre b = classify_pre_b<false>(P, rd, a, total_bytes);

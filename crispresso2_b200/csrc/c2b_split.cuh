@@ -568,106 +568,6 @@ C2B_DEV bool align_narrow16(const KParams &P, ASmem &S, const uint32_t *staged_p
     return true;
 }
 
-// ---------------------------------------------------------------------------------------- ALIGN, diagonal tier (tier 0)
-// A read as long as its amplicon whose ungapped score on the main diagonal beats every other path is aligned there, with no
-// DP: it scores strictly above RefDev::dg_thr4 (the bound on paths with an interior gap run, on offset diagonals past dg_S and
-// on paths through the reference's min_score borders) and strictly above the exact score of each offset diagonal 1..dg_S with
-// its two edge runs.  Then the diagonal is the unique optimum and the reference's traceback returns it (DESIGN.md section 3).
-// One read per warp, 32 consecutive reads per unit; the unit's unproved reads go, in order and with one atomic, on the tier-0
-// list (P.left0) that the narrow tier works through.
-struct DSmem {                                         // diagonal tier, per warp
-    uint8_t fw[RG_COMBO], rc[RG_COMBO];
-    uint8_t lut[256];
-    int64_t off[33];
-    int32_t ref[32];
-};
-
-// true if read rd is proved (op stream and meta word written); all lanes call with warp-uniform arguments
-C2B_DEV bool diag_read(const KParams &P, DSmem &S, int64_t rd, int64_t off, int J, int r)
-{
-    const int lane = wp::lane();
-    const RefDev &R = refdev(P, r);
-    const int I = R.I;
-    // the reads the narrow tier would take (one candidate reference, packed ring admissible), of the amplicon's length
-    if (!R.dg_ok || J != I || J > RG_COMBO || J + 32 > P.TS || J > R.pk_maxJ || I + J > PK_MAX_ALN) return false;
-    const bool bad = load_codes_a(P, S.lut, off, J, S.fw, S.rc);
-    wp::sync();
-    if (bad) return false;
-    const int mode = strand_mode(P, R, S.fw, J);
-    if (mode == 2) return false;                     // both strands: the DP decides which one
-    const uint8_t *c = mode == 1 ? S.rc : S.fw;
-    const int32_t *prof = R.prof;                    // [q][Ipad]: 4 x matrix[reference row][alphabet[q]]
-    const int Ipad = R.Ipad, dS = R.dg_S;
-    int acc[9];                                      // acc[s + 4]: 4 x ungapped score of read base k + s against reference row k
-#pragma unroll
-    for (int s = 0; s < 9; s++) acc[s] = 0;
-    for (int k = lane; k < I; k += 32) {
-        const int32_t *pk = prof + k;
-#pragma unroll
-        for (int s = -4; s <= 4; s++) {
-            const int j = k + s;
-            if ((s < 0 ? -s : s) <= dS && j >= 0 && j < J) acc[s + 4] += pk[(int)c[j] * Ipad];
-        }
-    }
-#pragma unroll
-    for (int s = 0; s < 9; s++)
-#pragma unroll
-        for (int d = 16; d >= 1; d >>= 1) acc[s] += wp::shfl_xor(acc[s], d);
-    bool proved = acc[4] > R.dg_thr4;
-#pragma unroll
-    for (int s = -4; s <= 4; s++)
-        if (s != 0 && (s < 0 ? -s : s) <= dS) proved = proved && acc[4] > acc[s + 4] + R.dg_c4[s + 4];
-    if (!proved) return false;
-    // what align_narrow16 writes for an all-M traceback of I columns: op words of 32 ops, OP_NONE (3) past the end
-    const int64_t slot = oslot(P, rd, r);
-    if (lane < 16 && lane < P.NW) {
-        const int rem = I - 32 * lane;
-        P.gops[slot * P.NW + lane] = rem >= 32 ? 0ull : rem <= 0 ? ~0ull : (~0ull << (2 * rem));
-    }
-    if (lane == 0) P.gmeta[slot] = gmeta_pack(I, mode == 1, GM_ALIGNED);
-    return true;
-}
-
-C2B_DEV void dsmem_init(const KParams &P, DSmem &S)
-{
-    for (int k = wp::lane(); k < 256; k += 32) S.lut[k] = P.lut[k];
-    wp::sync();
-}
-
-// reads 32u .. 32u+31: returns the number proved
-C2B_DEV int diag_unit(const KParams &P, DSmem &S, int64_t u)
-{
-    const int lane = wp::lane();
-    const int64_t first = 32 * u;
-    const int n = P.n_reads - first < 32 ? (int)(P.n_reads - first) : 32;
-    {
-        const int64_t rd = first + lane;
-        if (lane < n) { S.off[lane] = P.offsets[rd]; S.ref[lane] = P.ref_id ? P.ref_id[rd] : 0; }
-        if (lane == 0) S.off[n] = P.offsets[first + n];
-    }
-    wp::sync();
-#ifndef C2B_EMU
-    {                                                // the unit's bytes towards L2 (about 8 KB), one request per line
-        const int64_t b0 = S.off[0] & ~(int64_t)127, b1 = S.off[n];
-        for (int64_t a = b0 + (int64_t)lane * 128; a < b1; a += 32 * 128) asm volatile("prefetch.global.L2 [%0];" ::"l"(P.reads + a));
-    }
-#endif
-    uint32_t fail = 0;
-#pragma unroll 1
-    for (int x = 0; x < n; x++) {
-        const int64_t off = S.off[x];
-        if (!diag_read(P, S, first + x, off, (int)(S.off[x + 1] - off), S.ref[x])) fail |= 1u << x;
-        wp::sync();
-    }
-    if (fail) {                                      // warp-aggregated append: the unit's leftovers stay in read order
-        unsigned long long pos = 0;
-        if (lane == 0) pos = wp::fetch_add(P.left0_n, (unsigned long long)wp::popc(fail));
-        pos = (unsigned long long)(uint32_t)wp::shfl((int)(uint32_t)pos, 0) | ((unsigned long long)(uint32_t)wp::shfl((int)(uint32_t)(pos >> 32), 0) << 32);
-        if ((fail >> lane) & 1u) P.left0[pos + wp::popc(fail & ((1u << lane) - 1u))] = (int32_t)(first + lane);
-    }
-    return n - wp::popc(fail);
-}
-
 // ------------------------------------------------------------------------------------------------- CLASSIFY
 // One alignment per warp, one column per lane, 32 columns per step, left to right.  Column c (from the left) is op number
 // n-1-c of the stream (the walk emits right to left).  With bI / bJ the ballots of the insertion / deletion columns of a
@@ -1061,6 +961,88 @@ C2B_DEV void classify_stage(const BPre &b, BSmem &S)
     reinterpret_cast<uint4 *>(S.rd)[lane] = b.bytes;
 }
 
+// Pass 0's result for reference r (alignment of n columns on `strand`) -> the alignment record and the best-reference bookkeeping
+template <int NA>
+C2B_DEV void note_aln(c2b_read_rec &rec, c2b_aln_rec &a, const RefDev &R, int r, const ColOut &co, int n, int strand, ScAcc<NA> &A)
+{
+    init_aln(a, 0);
+    a.n_match = (uint16_t)co.n_match; a.aln_len = (uint16_t)n; a.strand = (uint8_t)strand;
+    a.score_milli = score_milli(co.n_match, n);
+    a.irregular_ends = (uint8_t)co.irregular;
+    note_score(rec, R, r, a.score_milli);
+    if ((unsigned)n > A.wmax) A.wmax = (unsigned)n;               // widest alignment of the launch
+}
+
+// The per-winner part of classify_read: reference r's alignment, a winner of read rd -> its alignment record, edit list,
+// count vectors and scalars.  scan(o, ed, mode) runs the alignment's column scan with colscan1's mode bits (RM_SCAL, RM_VEC,
+// RM_LEN); `a` is the record note_aln filled (used when the read has one candidate reference: multi reloads it).
+template <bool ONE, class Scan>
+C2B_DEV void classify_winner(const KParams &P, const RefDev &R, int64_t rd, int r, c2b_read_rec &rec, const c2b_aln_rec &a,
+                             bool multi, bool ambiguous, int nth, long long cnt, long long w, ScAcc<ONE ? 1 : RG_MAX_REFS> &A,
+                             const Scan &scan)
+{
+    const int lane = wp::lane();
+    const bool expand = P.flags & C2B_F_EXPAND_AMBIGUOUS, first = P.flags & C2B_F_ASSIGN_FIRST;
+    const bool ign_s = P.flags & C2B_F_IGNORE_SUBSTITUTIONS, ign_i = P.flags & C2B_F_IGNORE_INSERTIONS,
+               ign_d = P.flags & C2B_F_IGNORE_DELETIONS;
+    const bool two_scans = (P.flags & C2B_F_DISCARD_INDEL_READS) != 0;
+    rec.best_ref = (int16_t)r;                          // best_match_name = last winner (:768)
+    RowOut o; o.ins_n = o.del_n = o.sub_n = 0; o.n_ins_all = o.n_ins_win = o.n_del_all = o.n_del_win = 0;
+    o.n_del_pos = o.n_sub_all = 0; o.nent = 0;
+    c2b_edit *ed = P.edits ? P.edits + oslot(P, rd, r) * (int64_t)P.edit_cap : nullptr;
+    const bool counted = !ambiguous && (!first || nth == 0) && w > 0;
+    // with no ignore_* flag a window indel makes the read MODIFIED, so the length vectors (:4104-4115) can be updated in
+    // the same scan; otherwise (and under --discard_indel_reads) the scalars decide first
+    const bool len_inline = counted && !two_scans && !ign_i && !ign_d;
+    scan(o, ed, RM_SCAL | ((counted && !two_scans) ? RM_VEC : 0) | (len_inline ? RM_LEN : 0));
+    const bool has_d = !ign_d && o.del_n > 0, has_i = !ign_i && o.ins_n > 0, has_s = !ign_s && o.sub_n > 0;
+    const bool modified = has_d || has_i || has_s;     // CRISPRessoCORE.py:746-753 (same truth table)
+    uint32_t astatus = 0;
+    if (P.edits && o.nent > P.edit_cap) astatus |= C2B_ST_EDIT_OVERFLOW;
+    if (counted) {
+        const bool discard = two_scans && (o.del_n > 0 || o.ins_n > 0);
+        if (discard) sc_acc(A, P, r, C2B_S_DISCARDED, w);
+        else {
+            const bool entered = modified || R.tem != 0;
+            const bool lenv = !len_inline && entered && (o.n_ins_win > 0 || o.n_del_win > 0);
+            if (two_scans || lenv) scan(o, nullptr, (two_scans ? RM_VEC : 0) | (lenv ? RM_LEN : 0));
+            if (entered) edited_update_acc(A, P, R, r, o, w);              // references with a coding sequence never get here
+            sc_acc(A, P, r, C2B_S_TOTAL, w);
+            sc_acc(A, P, r, modified ? C2B_S_MODIFIED : C2B_S_UNMODIFIED, w);
+        }
+    } else if (ambiguous && nth == 0 && w > 0) sc_acc(A, P, r, C2B_S_AMBIGUOUS_W, w);
+    if (counted && (two_scans || expand)) {
+        const bool discarded = two_scans && (o.del_n > 0 || o.ins_n > 0), joined = !ONE && expand && !first && rec.n_winners > 1;   // assign-first is tested first (:780-785)
+        if (discarded != joined) sc_acc(A, P, r, modified ? C2B_S_CLASS_MODIFIED : C2B_S_CLASS_UNMODIFIED, discarded ? w : -w);
+    }
+    int irr = 0;
+    if (lane == 0) {
+        c2b_aln_rec b = multi ? load_aln(P.alns + oslot(P, rd, r)) : a;
+        b.insertion_n = (uint16_t)o.ins_n; b.deletion_n = (uint16_t)o.del_n; b.substitution_n = (uint16_t)o.sub_n;
+        b.n_ins_all = (uint16_t)o.n_ins_all; b.n_ins_win = (uint16_t)o.n_ins_win;
+        b.n_del_all = (uint16_t)o.n_del_all; b.n_del_win = (uint16_t)o.n_del_win;
+        b.n_del_pos_all = (uint16_t)o.n_del_pos; b.n_sub_all = (uint16_t)o.n_sub_all;
+        b.n_edits = (uint16_t)o.nent; b.modified = modified; b.status |= (uint8_t)astatus;
+        irr = b.irregular_ends;
+        P.alns[oslot(P, rd, r)] = b;
+    }
+    irr = wp::shfl(irr, 0);
+    rec.status |= astatus;
+    // aln_stats of the serial process_fastq branch use best_match_name only (:1971-1979): the LAST winner
+    const bool is_last = (rec.winner_mask >> (r & 31)) >> 1 == 0;
+    if (is_last) {
+        const long long total_mods = o.n_ins_all + o.n_del_pos + o.n_sub_all;
+        const long long in_win = o.sub_n + o.del_n + o.ins_n;
+        sc_acc(A, P, r, C2B_S_N_GLOBAL_SUBS, cnt * o.n_sub_all);
+        sc_acc(A, P, r, C2B_S_N_SUBS_OUTSIDE_WINDOW, cnt * (o.n_sub_all - o.sub_n));
+        sc_acc(A, P, r, C2B_S_N_MODS_IN_WINDOW, cnt * in_win);
+        sc_acc(A, P, r, C2B_S_N_MODS_OUTSIDE_WINDOW, cnt * (total_mods - in_win));
+        if (irr) sc_acc(A, P, r, C2B_S_N_READS_IRREGULAR_ENDS, cnt);
+        sc_acc(A, P, r, C2B_S_N_ALIGNED_UNIQUE, 1);
+        sc_acc(A, P, r, C2B_S_N_ALIGNED_COUNT, cnt);
+    }
+}
+
 template <bool ONE>
 C2B_DEV void classify_read(const KParams &P, int64_t rd, const BPre &pre, const BSmem &S, ScAcc<ONE ? 1 : RG_MAX_REFS> &A)
 {
@@ -1075,7 +1057,6 @@ C2B_DEV void classify_read(const KParams &P, int64_t rd, const BPre &pre, const 
     rec.ambiguous = 0; rec.status = 0;
     ColCtx cx[ONE ? 1 : RG_MAX_REFS];
     c2b_aln_rec a; init_aln(a, 0);
-    int keep_irr = 0;
 #pragma unroll 1
     for (int r = r_begin; r < r_end; r++) {
         const RefDev &R = refdev(P, r);
@@ -1085,13 +1066,7 @@ C2B_DEV void classify_read(const KParams &P, int64_t rd, const BPre &pre, const 
         c.ops = S.ops[ONE ? 0 : r - r_begin]; c.rd = S.rd + (int)((uintptr_t)(P.reads + off) & 15); c.n = (int)(gm & 0xffffu); c.J = J; c.strand = (int)((gm >> 16) & 1u);
         uint8_t *o_read = P.strings ? P.strings + (slot * 2) * (int64_t)P.W : nullptr;
         const ColOut co = colscan0(P, R, c, o_read, o_read ? o_read + P.W : nullptr);
-        init_aln(a, 0);
-        a.n_match = (uint16_t)co.n_match; a.aln_len = (uint16_t)c.n; a.strand = (uint8_t)c.strand;
-        a.score_milli = score_milli(co.n_match, c.n);
-        a.irregular_ends = (uint8_t)co.irregular;
-        keep_irr = co.irregular;
-        note_score(rec, R, r, a.score_milli);
-        if ((unsigned)c.n > A.wmax) A.wmax = (unsigned)c.n;           // widest alignment of the launch
+        note_aln(rec, a, R, r, co, c.n, c.strand, A);
         if (lane == 0 && multi) P.alns[slot] = a;
     }
     if (multi) wp::sync();
@@ -1103,73 +1078,16 @@ C2B_DEV void classify_read(const KParams &P, int64_t rd, const BPre &pre, const 
     const bool expand = P.flags & C2B_F_EXPAND_AMBIGUOUS, first = P.flags & C2B_F_ASSIGN_FIRST;
     const bool ambiguous = !ONE && rec.n_winners > 1 && !first && !expand;     // CRISPRessoCORE.py:780-785
     rec.ambiguous = ambiguous;
-    const long long cnt = pre.cnt;
     const long long w = pre.qw;
-    const bool ign_s = P.flags & C2B_F_IGNORE_SUBSTITUTIONS, ign_i = P.flags & C2B_F_IGNORE_INSERTIONS,
-               ign_d = P.flags & C2B_F_IGNORE_DELETIONS;
-    const bool two_scans = (P.flags & C2B_F_DISCARD_INDEL_READS) != 0;
     int nth = 0;
 #pragma unroll 1
     for (int r = r_begin; r < r_end; r++) {
         if (!((rec.winner_mask >> (r & 31)) & 1u)) continue;
         const RefDev &R = refdev(P, r);
         const ColCtx &c = cx[ONE ? 0 : r - r_begin];
-        rec.best_ref = (int16_t)r;                          // best_match_name = last winner (:768)
-        RowOut o; o.ins_n = o.del_n = o.sub_n = 0; o.n_ins_all = o.n_ins_win = o.n_del_all = o.n_del_win = 0;
-        o.n_del_pos = o.n_sub_all = 0; o.nent = 0;
-        c2b_edit *ed = P.edits ? P.edits + oslot(P, rd, r) * (int64_t)P.edit_cap : nullptr;
-        const bool counted = !ambiguous && (!first || nth == 0) && w > 0;
-        // with no ignore_* flag a window indel makes the read MODIFIED, so the length vectors (:4104-4115) can be updated in
-        // the same scan; otherwise (and under --discard_indel_reads) the scalars decide first
-        const bool len_inline = counted && !two_scans && !ign_i && !ign_d;
-        colscan1(P, R, c, o, ed, w, RM_SCAL | ((counted && !two_scans) ? RM_VEC : 0) | (len_inline ? RM_LEN : 0));
-        const bool has_d = !ign_d && o.del_n > 0, has_i = !ign_i && o.ins_n > 0, has_s = !ign_s && o.sub_n > 0;
-        const bool modified = has_d || has_i || has_s;     // CRISPRessoCORE.py:746-753 (same truth table)
-        uint32_t astatus = 0;
-        if (P.edits && o.nent > P.edit_cap) astatus |= C2B_ST_EDIT_OVERFLOW;
-        if (counted) {
-            const bool discard = two_scans && (o.del_n > 0 || o.ins_n > 0);
-            if (discard) sc_acc(A, P, r, C2B_S_DISCARDED, w);
-            else {
-                const bool entered = modified || R.tem != 0;
-                const bool lenv = !len_inline && entered && (o.n_ins_win > 0 || o.n_del_win > 0);
-                if (two_scans || lenv) colscan1(P, R, c, o, nullptr, w, (two_scans ? RM_VEC : 0) | (lenv ? RM_LEN : 0));
-                if (entered) edited_update_acc(A, P, R, r, o, w);              // references with a coding sequence never get here
-                sc_acc(A, P, r, C2B_S_TOTAL, w);
-                sc_acc(A, P, r, modified ? C2B_S_MODIFIED : C2B_S_UNMODIFIED, w);
-            }
-        } else if (ambiguous && nth == 0 && w > 0) sc_acc(A, P, r, C2B_S_AMBIGUOUS_W, w);
-        if (counted && (two_scans || expand)) {
-            const bool discarded = two_scans && (o.del_n > 0 || o.ins_n > 0), joined = !ONE && expand && !first && rec.n_winners > 1;   // assign-first is tested first (:780-785)
-            if (discarded != joined) sc_acc(A, P, r, modified ? C2B_S_CLASS_MODIFIED : C2B_S_CLASS_UNMODIFIED, discarded ? w : -w);
-        }
-        int irr = keep_irr;
-        if (lane == 0) {
-            c2b_aln_rec b = multi ? load_aln(P.alns + oslot(P, rd, r)) : a;
-            b.insertion_n = (uint16_t)o.ins_n; b.deletion_n = (uint16_t)o.del_n; b.substitution_n = (uint16_t)o.sub_n;
-            b.n_ins_all = (uint16_t)o.n_ins_all; b.n_ins_win = (uint16_t)o.n_ins_win;
-            b.n_del_all = (uint16_t)o.n_del_all; b.n_del_win = (uint16_t)o.n_del_win;
-            b.n_del_pos_all = (uint16_t)o.n_del_pos; b.n_sub_all = (uint16_t)o.n_sub_all;
-            b.n_edits = (uint16_t)o.nent; b.modified = modified; b.status |= (uint8_t)astatus;
-            irr = b.irregular_ends;
-            P.alns[oslot(P, rd, r)] = b;
-        }
-        irr = wp::shfl(irr, 0);
-        rec.status |= astatus;
+        classify_winner<ONE>(P, R, rd, r, rec, a, multi, ambiguous, nth, pre.cnt, w, A,
+                             [&](RowOut &o, c2b_edit *ed, int mode) { colscan1(P, R, c, o, ed, w, mode); });
         nth++;
-        // aln_stats of the serial process_fastq branch use best_match_name only (:1971-1979): the LAST winner
-        const bool is_last = (rec.winner_mask >> (r & 31)) >> 1 == 0;
-        if (is_last) {
-            const long long total_mods = o.n_ins_all + o.n_del_pos + o.n_sub_all;
-            const long long in_win = o.sub_n + o.del_n + o.ins_n;
-            sc_acc(A, P, r, C2B_S_N_GLOBAL_SUBS, cnt * o.n_sub_all);
-            sc_acc(A, P, r, C2B_S_N_SUBS_OUTSIDE_WINDOW, cnt * (o.n_sub_all - o.sub_n));
-            sc_acc(A, P, r, C2B_S_N_MODS_IN_WINDOW, cnt * in_win);
-            sc_acc(A, P, r, C2B_S_N_MODS_OUTSIDE_WINDOW, cnt * (total_mods - in_win));
-            if (irr) sc_acc(A, P, r, C2B_S_N_READS_IRREGULAR_ENDS, cnt);
-            sc_acc(A, P, r, C2B_S_N_ALIGNED_UNIQUE, 1);
-            sc_acc(A, P, r, C2B_S_N_ALIGNED_COUNT, cnt);
-        }
     }
     // HDR / prime editing: reads assigned to another reference are also classified on their alignment to reference 0
     if (!ONE && (P.flags & C2B_F_HDR_REF1) && multi && r_begin == 0 && !ambiguous && w > 0) {
@@ -1186,6 +1104,194 @@ C2B_DEV void classify_read(const KParams &P, int64_t rd, const BPre &pre, const 
         }
     }
     if (lane == 0) P.recs[rd] = rec;
+}
+
+// ---------------------------------------------------------------------------------------- diagonal tier (tier 0)
+// A read as long as its amplicon whose ungapped score on the main diagonal beats every other path is aligned there, with no
+// DP: it scores strictly above RefDev::dg_thr4 (the bound on paths with an interior gap run, on offset diagonals past dg_S and
+// on paths through the reference's min_score borders) and strictly above the exact score of each offset diagonal 1..dg_S with
+// its two edge runs.  Then the diagonal is the unique optimum and the reference's traceback returns it (DESIGN.md section 3).
+// The tier also classifies the reads it proves (diag_classify), so the narrow tier and CLASSIFY only see the others.
+// One read per warp, 32 consecutive reads per unit; the unit's unproved reads go, in order and with one atomic, on the tier-0
+// list (P.left0) that the narrow tier and CLASSIFY work through.
+struct DSmem {                                         // diagonal tier, per warp
+    uint8_t fw[RG_COMBO], rc[RG_COMBO];
+    uint8_t lut[256];
+    int64_t off[33];
+    int32_t ref[32], cnt[32], qw[32];
+};
+
+// classify_read<true> for a read the tier proved: I columns of OP_M on the main diagonal, no gap column.  c: the read as
+// alphabet codes in the aligned strand; column p's read character is P.alpha[c[p]], which is how col_decode spells it (the
+// lookup table maps exactly the alphabet's characters, and a read with any other symbol is never proved).
+C2B_DEV void diag_classify(const KParams &P, const DSmem &S, const RefDev &R, const uint8_t *c, int64_t rd, int r, int strand,
+                           long long cnt, long long w, ScAcc<1> &A)
+{
+    const int lane = wp::lane(), I = R.I;
+    const uint32_t lt = (1u << lane) - 1u;
+    const int64_t slot = oslot(P, rd, r);
+    const int nsteps = (I + 31) >> 5;
+    // pass 0 (colscan0): the two strings right-aligned in their W-byte slots, matchCount, irregular ends; lane m keeps the
+    // ballot of step m's mismatching columns
+    uint8_t *o_read = P.strings ? P.strings + (slot * 2) * (int64_t)P.W + P.W - I : nullptr;
+    int match = 0;
+    uint32_t irr = 0, mmis = 0;
+#pragma unroll 1
+    for (int m = 0; m < nsteps; m++) {
+        const int p = 32 * m + lane;
+        const bool valid = p < I;
+        const uint32_t rdc = valid ? P.alpha[c[p]] : 0u, rfc = valid ? R.asc[p] : 0u;
+        const uint32_t Bmis = wp::ballot(valid && rdc != rfc);
+        match += wp::popc(wp::ballot(valid && rdc == rfc));
+        irr |= wp::ballot(valid && (p == 0 || p == I - 1) && rdc != rfc);
+        if (o_read && valid) { o_read[p] = (uint8_t)rdc; o_read[P.W + p] = (uint8_t)rfc; }
+        if (lane == m) mmis = Bmis;
+    }
+    ColOut co; co.n_match = match; co.irregular = irr != 0;
+    c2b_read_rec rec; rec.winner_mask = 0; rec.best_score_milli = -1000; rec.best_ref = -1; rec.n_winners = 0;
+    rec.ambiguous = 0; rec.status = 0;
+    c2b_aln_rec a;
+    note_aln(rec, a, R, r, co, I, strand, A);
+    if (rec.best_score_milli <= 0) {
+        rec.winner_mask = 0; rec.n_winners = 0;
+        if (lane == 0) { P.alns[slot] = a; P.recs[rd] = rec; }
+        return;
+    }
+    // colscan1 without gap columns: every differing column is a substitution unless the read has N there; no runs, no flanks
+    auto scan = [&](RowOut &o, c2b_edit *ed, int mode) {
+        const bool scal = mode & RM_SCAL, vec = mode & RM_VEC, ign_s = P.flags & C2B_F_IGNORE_SUBSTITUTIONS;
+        unsigned long long *V = R.vec;
+        const int vs = P.vstride;
+#pragma unroll 1
+        for (int m = 0; m < nsteps; m++) {
+            const uint32_t bm = wp::shflu(mmis, m);
+            if (!bm) continue;                                                       // the read equals the reference here
+            const int p = 32 * m + lane;
+            const bool differs = (bm >> lane) & 1u;
+            const uint32_t rdc = differs ? P.alpha[c[p]] : 0u;
+            const bool issub = differs && rdc != 'N';                                // COREResources.pyx:111
+            const bool inc_p = differs && (R.incl[p] & 1u);
+            const int rcode = differs ? S.lut[rdc] : 0;
+            if (scal) {
+                const uint32_t Bs = wp::ballot(issub), Bsw = wp::ballot(issub && inc_p);
+                o.n_sub_all += wp::popc(Bs); o.sub_n += wp::popc(Bsw);
+                if (Bs) {
+                    const int idx = o.nent + wp::popc(Bs & lt);
+                    if (issub && idx < P.edit_cap && ed) {
+                        c2b_edit e; e.a = (uint16_t)p; e.b = 0; e.type = 1; e.in_window = inc_p; e.base = (uint8_t)rdc; e.pad = 0;
+                        ed[idx] = e;
+                    }
+                    o.nent += wp::popc(Bs);
+                }
+            }
+            if (vec) {
+                if (issub) {
+                    wp::addg(V + (int64_t)C2B_V_ALL_SUB * vs + p, w);
+                    if (!ign_s) {
+                        wp::addg(V + (int64_t)(C2B_V_SUBBASE0 + rcode) * vs + p, w);
+                        if (inc_p) wp::addg(V + (int64_t)C2B_V_SUB * vs + p, w);
+                    }
+                }
+                if (differs) {                                   // all_base_count_vectors as deviation from "read == ref"
+                    const int rc = R.rcode[p];
+                    wp::addg(V + (int64_t)(C2B_V_BASEDEV0 + rcode) * vs + p, w);
+                    if (rc != 255) wp::addg(V + (int64_t)(C2B_V_BASEDEV0 + rc) * vs + p, -w);
+                }
+            }
+        }
+    };
+    classify_winner<true>(P, R, rd, r, rec, a, false, false, 0, cnt, w, A, scan);
+    if (lane == 0) P.recs[rd] = rec;
+}
+
+// true if read rd is proved (op stream, meta word and classification written); all lanes call with warp-uniform arguments
+C2B_DEV bool diag_read(const KParams &P, DSmem &S, int64_t rd, int64_t off, int J, int r, long long cnt, long long w, ScAcc<1> &A)
+{
+    const int lane = wp::lane();
+    const RefDev &R = refdev(P, r);
+    const int I = R.I;
+    // the reads the narrow tier would take (one candidate reference, packed ring admissible), of the amplicon's length
+    if (!R.dg_ok || J != I || J > RG_COMBO || J + 32 > P.TS || J > R.pk_maxJ || I + J > PK_MAX_ALN) return false;
+    const bool bad = load_codes_a(P, S.lut, off, J, S.fw, S.rc);
+    wp::sync();
+    if (bad) return false;
+    const int mode = strand_mode(P, R, S.fw, J);
+    if (mode == 2) return false;                     // both strands: the DP decides which one
+    const uint8_t *c = mode == 1 ? S.rc : S.fw;
+    const int32_t *prof = R.prof;                    // [q][Ipad]: 4 x matrix[reference row][alphabet[q]]
+    const int Ipad = R.Ipad, dS = R.dg_S;
+    int acc[9];                                      // acc[s + 4]: 4 x ungapped score of read base k + s against reference row k
+#pragma unroll
+    for (int s = 0; s < 9; s++) acc[s] = 0;
+    for (int k = lane; k < I; k += 32) {
+        const int32_t *pk = prof + k;
+#pragma unroll
+        for (int s = -4; s <= 4; s++) {
+            const int j = k + s;
+            if ((s < 0 ? -s : s) <= dS && j >= 0 && j < J) acc[s + 4] += pk[(int)c[j] * Ipad];
+        }
+    }
+#pragma unroll
+    for (int s = 0; s < 9; s++)
+#pragma unroll
+        for (int d = 16; d >= 1; d >>= 1) acc[s] += wp::shfl_xor(acc[s], d);
+    bool proved = acc[4] > R.dg_thr4;
+#pragma unroll
+    for (int s = -4; s <= 4; s++)
+        if (s != 0 && (s < 0 ? -s : s) <= dS) proved = proved && acc[4] > acc[s + 4] + R.dg_c4[s + 4];
+    if (!proved) return false;
+    // what align_narrow16 writes for an all-M traceback of I columns: op words of 32 ops, OP_NONE (3) past the end
+    const int64_t slot = oslot(P, rd, r);
+    if (lane < 16 && lane < P.NW) {
+        const int rem = I - 32 * lane;
+        P.gops[slot * P.NW + lane] = rem >= 32 ? 0ull : rem <= 0 ? ~0ull : (~0ull << (2 * rem));
+    }
+    if (lane == 0) P.gmeta[slot] = gmeta_pack(I, mode == 1, GM_ALIGNED);
+    diag_classify(P, S, R, c, rd, r, mode == 1, cnt, w, A);
+    return true;
+}
+
+C2B_DEV void dsmem_init(const KParams &P, DSmem &S)
+{
+    for (int k = wp::lane(); k < 256; k += 32) S.lut[k] = P.lut[k];
+    wp::sync();
+}
+
+// reads 32u .. 32u+31: returns the number proved; A: the warp's scalar accumulators (flushed by the caller)
+C2B_DEV int diag_unit(const KParams &P, DSmem &S, int64_t u, ScAcc<1> &A)
+{
+    const int lane = wp::lane();
+    const int64_t first = 32 * u;
+    const int n = P.n_reads - first < 32 ? (int)(P.n_reads - first) : 32;
+    {
+        const int64_t rd = first + lane;
+        if (lane < n) {
+            S.off[lane] = P.offsets[rd]; S.ref[lane] = P.ref_id ? P.ref_id[rd] : 0;
+            S.cnt[lane] = P.count ? P.count[rd] : 1; S.qw[lane] = P.qweight ? P.qweight[rd] : S.cnt[lane];
+        }
+        if (lane == 0) S.off[n] = P.offsets[first + n];
+    }
+    wp::sync();
+#ifndef C2B_EMU
+    {                                                // the unit's bytes towards L2 (about 8 KB), one request per line
+        const int64_t b0 = S.off[0] & ~(int64_t)127, b1 = S.off[n];
+        for (int64_t a = b0 + (int64_t)lane * 128; a < b1; a += 32 * 128) asm volatile("prefetch.global.L2 [%0];" ::"l"(P.reads + a));
+    }
+#endif
+    uint32_t fail = 0;
+#pragma unroll 1
+    for (int x = 0; x < n; x++) {
+        const int64_t off = S.off[x];
+        if (!diag_read(P, S, first + x, off, (int)(S.off[x + 1] - off), S.ref[x], S.cnt[x], S.qw[x], A)) fail |= 1u << x;
+        wp::sync();
+    }
+    if (fail) {                                      // warp-aggregated append: the unit's leftovers stay in read order
+        unsigned long long pos = 0;
+        if (lane == 0) pos = wp::fetch_add(P.left0_n, (unsigned long long)wp::popc(fail));
+        pos = (unsigned long long)(uint32_t)wp::shfl((int)(uint32_t)pos, 0) | ((unsigned long long)(uint32_t)wp::shfl((int)(uint32_t)(pos >> 32), 0) << 32);
+        if ((fail >> lane) & 1u) P.left0[pos + wp::popc(fail & ((1u << lane) - 1u))] = (int32_t)(first + lane);
+    }
+    return n - wp::popc(fail);
 }
 
 }  // namespace c2b

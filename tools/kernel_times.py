@@ -4,7 +4,10 @@ Runs the workload under torch.profiler (CUDA activity only, nothing else timed i
 time per launch of every kernel by name, the launch order of one step, the diagonal tier's read counts per step and
 the card with its power limit: means over the profiled steps.
 
-  python tools/kernel_times.py [--reads 1048576] [--steps 20] [--warmup 3] [--json OUT]
+  python tools/kernel_times.py [--reads 1048576] [--steps 20] [--warmup 3] [--mix bench|proved|unproved] [--json OUT]
+
+--mix replaces the bench's reads (same amplicon, same count): `proved` = reads as long as the amplicon with 0-2
+substitutions and no gap (what the diagonal tier proves), `unproved` = the bench's deletion and insertion templates only.
 """
 import argparse
 import json
@@ -28,11 +31,32 @@ def card_info(index):
         return {"name": None, "error": str(exc)}
 
 
+def mix_reads(mix, ref, n):
+    """[n, 250] uint8 reads of --mix `proved` / `unproved` against the bench amplicon (fixed seed)"""
+    import numpy as np
+    from crispresso2_b200 import synth
+    rng = np.random.default_rng(2024)
+    amp = ref["sequence"]
+    if mix == "unproved":                        # the bench's deletion (25 %) and insertion (10 %) templates, nothing else
+        return synth.synth_reads_fast(rng, amp, n, 250, del_frac=0.25 / 0.35, ins_frac=0.10 / 0.35, cut=ref["cut_point"])
+    acgt = np.frombuffer(b"ACGT", dtype=np.uint8)
+    out = np.tile(np.frombuffer(amp.encode(), dtype=np.uint8), (n, 1))
+    for k in range(2):                           # 0, 1 or 2 substitutions per read, each to a different base
+        rows = np.nonzero(rng.integers(0, 3, size=n) > k)[0]
+        cols = rng.integers(0, out.shape[1], size=len(rows))
+        old = out[rows, cols]
+        new = acgt[rng.integers(0, 4, size=len(rows))]
+        new = np.where(new == old, acgt[(np.searchsorted(acgt, new) + 1) % 4], new)
+        out[rows, cols] = new
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reads", type=int, default=1 << 20)
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--mix", default="bench", choices=["bench", "proved", "unproved"])
     ap.add_argument("--json", help="also write the table as JSON here")
     args = ap.parse_args()
 
@@ -49,6 +73,8 @@ def main():
     w = Workload("single", n, 0)
     eng = Engine(0)
     P = w.params
+    if args.mix != "bench":
+        w.buf = mix_reads(args.mix, w.refs["Reference"], n).reshape(-1)
     eng.configure(w.refs, w.ref_names, O.make_matrix(), P.needleman_wunsch_gap_open, P.needleman_wunsch_gap_extend,
                   P.aln_seed_count, P.aln_seed_min, w.flags, "ACGTN", 12)
     W = eng.string_width(w.max_len)
@@ -111,8 +137,8 @@ def main():
             diag = {"proved": a.value // args.steps, "tier1": b.value // args.steps, "tier2": c.value // args.steps}
     info = card_info(0)
     print("card: %s, power limit %s W, max SM clock %s MHz" % (info.get("name"), info.get("power_limit_w"), info.get("max_sm_clock_mhz")))
-    print("%d reads x 250 bp, %d profiled steps after %d warm-up steps; C2B_NO_DIAG=%s" % (n, args.steps, args.warmup,
-                                                                                      os.environ.get("C2B_NO_DIAG", "")))
+    print("%d reads x 250 bp (mix %s), %d profiled steps after %d warm-up steps; C2B_NO_DIAG=%s" % (
+        n, args.mix, args.steps, args.warmup, os.environ.get("C2B_NO_DIAG", "")))
     print("| # | kernel | ms / launch | share |")
     print("|---|---|---|---|")
     for r in rows:
@@ -123,7 +149,7 @@ def main():
               (diag["proved"], 100.0 * diag["proved"] / n, diag["tier1"], diag["tier2"]))
     if args.json:
         with open(args.json, "w") as fh:
-            json.dump({"card": info, "reads": n, "steps": args.steps, "no_diag": os.environ.get("C2B_NO_DIAG", ""),
+            json.dump({"card": info, "reads": n, "steps": args.steps, "mix": args.mix, "no_diag": os.environ.get("C2B_NO_DIAG", ""),
                        "kernels": rows, "total_ms_per_step": total, "diag_counts": diag}, fh, indent=1)
 
 
