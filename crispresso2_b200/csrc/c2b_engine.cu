@@ -352,6 +352,7 @@ __global__ void __launch_bounds__(B_WARPS_PER_CTA * 32, C2B_B_MIN_CTAS) c2b_clas
 struct RefHost {
     std::string seq; std::vector<int64_t> gi, inc; double min_aln; std::vector<int64_t> rows;
     std::vector<std::string> fw, rc;
+    int64_t sabs = 0, gabs = 0, gsum_abs = 0, gi0_abs = 0;   // largest |score|, largest and summed |gap_incentive|, |gap_incentive[0]|
 };
 
 struct DevBuf {
@@ -659,6 +660,12 @@ int c2b_configure(c2b_engine *e, const c2b_params *p, int32_t n_refs, const c2b_
                 prof[(size_t)q * Ipad + i] = (int32_t)(4 * v);
             }
         for (int i = 0; i <= I; i++) if (rf.gap_incentive[i] > lim || rf.gap_incentive[i] < -lim) return fail(e, C2B_E_LIMIT, "c2b_configure: gap incentive out of range");
+        {   // extrema for the per-batch score range check (score_range_ok)
+            RefHost &h = e->refs[r];
+            h.sabs = h.gabs = h.gsum_abs = 0; h.gi0_abs = std::abs(rf.gap_incentive[0]);
+            for (size_t k = 0; k < (size_t)p->nq * I; k++) h.sabs = std::max<int64_t>(h.sabs, std::abs(rf.score_rows[k]));
+            for (int i = 0; i <= I; i++) { h.gabs = std::max<int64_t>(h.gabs, std::abs(rf.gap_incentive[i])); h.gsum_abs += std::abs(rf.gap_incentive[i]); }
+        }
         for (int row = 0; row < I; row++) {
             cIe[row] = (int32_t)(4 * (p->gap_extend + rf.gap_incentive[row + 1]));
             g4[row] = (int32_t)(4 * rf.gap_incentive[row]);
@@ -863,6 +870,24 @@ static int ensure_scratch(c2b_engine *e, int maxJ)
     return C2B_OK;
 }
 
+// Every DP value is stored as 4 * score + tag in int32, where the reference keeps the raw score in a C int: refuse a batch whose
+// scores could wrap here while the reference still computes them exactly.  A cell of reference r's matrix for reads up to maxJ
+// holds a path score from the origin or from a min_score border (gap_open * I * J).  On the way there are at most min(I, J)
+// substitutions and I + J gap columns, each with one gap_open or gap_extend term; an inserted read base adds its row's
+// incentive (at most J of them), an opened deletion that of the row it leaves (distinct rows), a border cell gap_incentive[0].
+static int score_range_ok(c2b_engine *e, int64_t maxJ, const char *who)
+{
+    const int64_t go = std::abs((int64_t)e->prm.gap_open), gap = std::max(go, std::abs((int64_t)e->prm.gap_extend));
+    for (int r = 0; r < e->n_refs; r++) {
+        const RefHost &h = e->refs[r];
+        const int64_t I = (int64_t)h.seq.size(), J = std::max<int64_t>(maxJ, 1);
+        const int64_t bound = go * I * J + std::min(I, J) * h.sabs + (I + J) * gap + J * h.gabs + h.gsum_abs + h.gi0_abs;
+        if (4 * bound + 3 > (int64_t)INT32_MAX)
+            return fail(e, C2B_E_LIMIT, std::string(who) + ": scores, gap penalties and incentives can exceed the int32 range of the DP");
+    }
+    return C2B_OK;
+}
+
 // One batch on compute stream `cs` using scratch set `set` (0 or 1): the ALIGN / CLASSIFY pair followed by the general
 // kernel over what ALIGN left over -- or the general kernel alone where the two-kernel form does not apply.  Launches that
 // may overlap in time must use different sets; launches on the same stream are ordered.
@@ -881,6 +906,7 @@ static int launch_on(c2b_engine *e, rt_stream cs, int set, const uint8_t *d_read
     if (max_read_len > C2B_MAX_READ_LEN) return fail(e, C2B_E_LIMIT, "c2b_align_batch: read longer than C2B_MAX_READ_LEN");
     if ((int64_t)std::abs((long long)e->prm.gap_open) * max_read_len * e->max_I >= (1ll << 28))
         return fail(e, C2B_E_LIMIT, "c2b_align_batch: gap_open * lengths exceeds the int32 score range");
+    if (int rc0 = score_range_ok(e, max_read_len, "c2b_align_batch")) return rc0;
     if (!d_ref_id && e->n_refs > C2B_MAX_REFS)
         return fail(e, C2B_E_LIMIT, "c2b_align_batch: more than C2B_MAX_REFS references need a per-read ref_id");
     int rc = ensure_scratch(e, max_read_len);
@@ -1227,6 +1253,7 @@ static int align_batch_host(c2b_engine *e, const uint8_t *reads, const int64_t *
     }
     if (minJ < 0) return fail(e, C2B_E_ARG, "c2b_align_batch: offsets not monotone");
     if (maxJ > C2B_MAX_READ_LEN) return fail(e, C2B_E_LIMIT, "c2b_align_batch: read longer than C2B_MAX_READ_LEN");
+    if (int rc0 = score_range_ok(e, maxJ, "c2b_align_batch")) return rc0;     // before anything is queued
     if (!e->pipe_ready) {
         RTCHK(rt_stream_create(&e->s_in));
         RTCHK(rt_stream_create(&e->s_out));

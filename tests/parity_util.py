@@ -213,14 +213,14 @@ def check_seed_disagreement(engine, n=1536):
     return sum(1 for m in modes if len(set(m)) > 1)
 
 
-def check_pooled(engine, n_amplicons=6, reads_per=40, seed=21, amp_len=(120, 200)):
+def check_pooled(engine, n_amplicons=6, reads_per=40, seed=21, amp_len=(120, 200), matrix=None, go=-20, ge=-2):
     """Config-4 shape (post-demultiplex Pooled): every read carries the index of its single amplicon (ref_id).
     Each (amplicon, read) must equal what the oracle computes with that amplicon alone; the count block of
-    amplicon k must equal the oracle's single-amplicon quantification of k's reads."""
+    amplicon k must equal the oracle's single-amplicon quantification of k's reads.  matrix / go / ge replace EDNAFULL, -20 / -2."""
     from crispresso2_b200 import synth, core
     from crispresso2_b200.engine import pack_reads
     rng = np.random.default_rng(seed)
-    m = O.make_matrix()
+    m = O.make_matrix() if matrix is None else matrix
     refs, names, reads, rid = {}, [], [], []
     for k in range(n_amplicons):
         L = int(rng.integers(amp_len[0], amp_len[1] + 1))
@@ -234,11 +234,11 @@ def check_pooled(engine, n_amplicons=6, reads_per=40, seed=21, amp_len=(120, 200
     order = rng.permutation(len(reads))
     reads = [reads[i] for i in order]
     rid = [rid[i] for i in order]
-    engine.configure(refs, names, m, -20, -2, 5, 2, 0, "ACGTN", 64)
+    engine.configure(refs, names, m, go, ge, 5, 2, 0, "ACGTN", 64)
     engine.counts_reset()
     buf, off = pack_reads(reads)
     res = engine.align_packed(buf, off, ref_id=np.asarray(rid, dtype=np.int32))
-    params = O.Params()
+    params = O.Params(needleman_wunsch_gap_open=go, needleman_wunsch_gap_extend=ge)
     per_amp = {k: [] for k in range(n_amplicons)}
     for i, s in enumerate(reads):
         k = rid[i]
@@ -349,17 +349,22 @@ def check_legacy(engine, n=120, seed=17):
     check_against_oracle(engine, {"Reference": ref, "HDR": ref2}, ["Reference", "HDR"], P, reads[:60] + r2 + reads[-10:], O.make_matrix())
 
 
-def check_narrow_equals_wide(engine, n=640, I=250, seed=59, oracle_subset=0):
+def check_narrow_equals_wide(engine, n=640, I=250, seed=59, oracle_subset=0, matrix=None, go=-20, ge=-2, gap_incentive=None):
     """Narrow first tier of the ALIGN kernel (sixteen reads per warp, band of 36 slots, result kept iff the score beats that
     band's bound; everything else re-queued for the 72-slot ring / the full matrix) against the same batch with the tier
     switched off (C2B_NO_NARROW): identical records, op streams, strings, edit lists and count block.  Reads straddle the narrow
-    bound: deletions of 1..24 bp, insertions of 1..16 bp, 0..40 substitutions, reverse-complemented and both-strand reads."""
+    bound: deletions of 1..24 bp, insertions of 1..16 bp, 0..40 substitutions, reverse-complemented and both-strand reads.
+    matrix / go / ge / gap_incentive (an I + 1 array) replace EDNAFULL, -20 / -2 and the cut-site incentive.
+    -> diag_counts() of the run with the tier"""
     import os
     from crispresso2_b200 import synth
     from crispresso2_b200.engine import pack_reads
     rng = np.random.default_rng(seed)
     amp = synth.random_amplicon(rng, I)
     ref = synth.amplicon_setup(amp, guide_start=max(1, I // 2 - 10))
+    m = O.make_matrix() if matrix is None else matrix
+    if gap_incentive is not None:
+        ref["gap_incentive"] = np.asarray(gap_incentive, dtype=np.int64)
     acgt = list("ACGT")
     comp = {"A": "T", "C": "G", "G": "C", "T": "A", "N": "N"}
     reads = []
@@ -389,14 +394,15 @@ def check_narrow_equals_wide(engine, n=640, I=250, seed=59, oracle_subset=0):
         if off_switch:
             os.environ["C2B_NO_NARROW"] = off_switch
         try:
-            engine.configure({"Reference": ref}, ["Reference"], O.make_matrix(), -20, -2, 5, 2, 0, "ACGTN", 48)
+            engine.configure({"Reference": ref}, ["Reference"], m, go, ge, 5, 2, 0, "ACGTN", 48)
             engine.counts_reset()
             res = engine.align_packed(buf, off)
+            dc = engine.diag_counts()
             cres = engine.align_packed(buf, off, compact=True, count=np.zeros(n, dtype=np.int32), qweight=np.zeros(n, dtype=np.int32))
-            out.append((res, engine.counts_raw(), cres))
+            out.append((res, engine.counts_raw(), cres, dc))
         finally:
             os.environ.pop("C2B_NO_NARROW", None)
-    (a, ca, xa), (b, cb, xb) = out
+    (a, ca, xa, da), (b, cb, xb, _) = out
     assert (a.recs == b.recs).all() and (a.alns == b.alns).all() and (ca == cb).all()
     assert ((xa.meta & 0xffffff) == (xb.meta & 0xffffff)).all() and (((xa.meta >> 24) != 0) == ((xb.meta >> 24) != 0)).all()   # columns, strand; the state byte names the kernel that aligned
     W = a.W
@@ -409,7 +415,9 @@ def check_narrow_equals_wide(engine, n=640, I=250, seed=59, oracle_subset=0):
         used = (int(nw[k]) + 31) // 32
         assert (xa.ops.reshape(n, -1)[k, :used] == xb.ops.reshape(n, -1)[k, :used]).all(), k
     if oracle_subset:
-        check_against_oracle(engine, {"Reference": ref}, ["Reference"], O.Params(), reads[:oracle_subset], O.make_matrix())
+        check_against_oracle(engine, {"Reference": ref}, ["Reference"], O.Params(needleman_wunsch_gap_open=go, needleman_wunsch_gap_extend=ge),
+                             reads[:oracle_subset], m)
+    return da
 
 
 def check_long_pairs(engine, n=40, seed=91):
@@ -436,16 +444,20 @@ def check_long_pairs(engine, n=40, seed=91):
         assert singles <= 8 and pairs > 0, (I, J, pairs, singles)      # the last, incomplete group of eight goes to the general kernel
 
 
-def check_ring_equals_full(engine, n=96, I=250, seed=41, oracle_subset=0):
+def check_ring_equals_full(engine, n=96, I=250, seed=41, oracle_subset=0, matrix=None, go=-20, ge=-2, gap_incentive=None):
     """Ring-banded DP (four pairs per warp, only a diagonal band computed, result kept iff the score beats the
     out-of-band bound) against the full-matrix packed path: identical records, alignments, strings, edit lists and
     count block.  Reads are built to straddle the bound: deletions of 1..48 bp, insertions of 1..40 bp, heavy
-    substitution loads, random reads."""
+    substitution loads, random reads.  matrix / go / ge / gap_incentive (an I + 1 array) replace EDNAFULL, -20 / -2 and the
+    cut-site incentive."""
     from crispresso2_b200 import synth, _lib
     from crispresso2_b200.engine import pack_reads
     rng = np.random.default_rng(seed)
     amp = synth.random_amplicon(rng, I)
     ref = synth.amplicon_setup(amp, guide_start=max(1, I // 2 - 10))
+    m = O.make_matrix() if matrix is None else matrix
+    if gap_incentive is not None:
+        ref["gap_incentive"] = np.asarray(gap_incentive, dtype=np.int64)
     acgt = list("ACGT")
     reads = []
     for k in range(n):
@@ -472,7 +484,7 @@ def check_ring_equals_full(engine, n=96, I=250, seed=41, oracle_subset=0):
     buf, off = pack_reads(reads)
     out = []
     for flags in (0, _lib.F_NO_RING):
-        engine.configure({"Reference": ref}, ["Reference"], O.make_matrix(), -20, -2, 5, 2, flags, "ACGTN", 40)
+        engine.configure({"Reference": ref}, ["Reference"], m, go, ge, 5, 2, flags, "ACGTN", 40)
         engine.counts_reset()
         res = engine.align_packed(buf, off)
         pc = engine.path_counts()
@@ -487,7 +499,8 @@ def check_ring_equals_full(engine, n=96, I=250, seed=41, oracle_subset=0):
     (ea, fa), (eb, fb) = edits_canonical(a), edits_canonical(b)
     assert (fa == fb).all() and (ea[fa] == eb[fb]).all()
     if oracle_subset:
-        check_against_oracle(engine, {"Reference": ref}, ["Reference"], O.Params(), reads[:oracle_subset], O.make_matrix())
+        check_against_oracle(engine, {"Reference": ref}, ["Reference"], O.Params(needleman_wunsch_gap_open=go, needleman_wunsch_gap_extend=ge),
+                             reads[:oracle_subset], m)
     return ra
 
 

@@ -120,11 +120,17 @@ def _cases(tmp=None):
         # annotates every FASTQ record from variantCache / not_aligned -- with the engine's lazy entries behind it
         "fanc_fastq_output": ["-r1", fq, "-a", ns["FANC"], "-g", g, "-e", ns["FANC_HDR"], "--fastq_output"],
         "fanc_legacy": ["-r1", fq, "-a", ns["FANC"], "-g", g, "-e", ns["FANC_HDR"], "--use_legacy_insertion_quantification", "-w", "4"],
+        # scoring options: an asymmetric NCBI-format matrix (tests/golden/scoring_nuc.matrix), gap_open == gap_extend, incentive 3
+        "fanc_scoring": ["-r1", fq, "-a", ns["FANC"], "-g", g] + SCORING_ARGS,
     }
 
 
+SCORING_ARGS = ["--needleman_wunsch_aln_matrix_loc", os.path.join(HERE, "golden", "scoring_nuc.matrix"),
+                "--needleman_wunsch_gap_open", "-6", "--needleman_wunsch_gap_extend", "-6", "--needleman_wunsch_gap_incentive", "3"]
+
+
 @pytest.mark.parametrize("case", ["fanc_default", "fanc_params", "fanc_flags", "fanc_fastq_output", "fanc_legacy", "fanc_pe_scaffold",
-                                  "fanc_pe_scaffold_discard", "fanc_paired_merge", "fanc_paired_merge_out"])
+                                  "fanc_pe_scaffold_discard", "fanc_paired_merge", "fanc_paired_merge_out", "fanc_scoring"])
 def test_reference_cli_with_engine_process_fastq_is_byte_identical(case, tmp_path):
     import build_emu
     lib = build_emu.build()

@@ -57,8 +57,9 @@ def device_batch(engine, reads, ref_id, cap=48):
     return get()
 
 
-def run_both(engine, refs, names, reads, go=-20, ge=-2, flags=0, ref_id=None):
-    """-> diag_counts of the default run; asserts that the run without the tier computed the same."""
+def run_both(engine, refs, names, reads, go=-20, ge=-2, flags=0, ref_id=None, matrix=None):
+    """-> diag_counts of the default run; asserts that the run without the tier computed the same.  matrix: EDNAFULL if None."""
+    m = O.make_matrix() if matrix is None else matrix
     buf, off = pack_reads(reads)
     n = len(reads)
     out = []
@@ -66,7 +67,7 @@ def run_both(engine, refs, names, reads, go=-20, ge=-2, flags=0, ref_id=None):
         if switch:
             os.environ["C2B_NO_DIAG"] = switch
         try:
-            engine.configure(refs, names, O.make_matrix(), go, ge, 5, 2, flags, "ACGTN", 48)
+            engine.configure(refs, names, m, go, ge, 5, 2, flags, "ACGTN", 48)
             engine.counts_reset()
             res = engine.align_packed(buf, off, ref_id=ref_id)
             dc = engine.diag_counts()
@@ -93,10 +94,10 @@ def run_both(engine, refs, names, reads, go=-20, ge=-2, flags=0, ref_id=None):
     return da
 
 
-def rule_count(reads, refs, names, go=-20, ge=-2, ref_id=None, alphabet="ACGTN"):
+def rule_count(reads, refs, names, go=-20, ge=-2, ref_id=None, alphabet="ACGTN", matrix=None):
     """The proof rule restated on the host: reads of the amplicon's length, every base in the alphabet, one strand from the
     seed test, strictly above the bound on the other path classes and above the exact scores of the near offset diagonals."""
-    m = O.make_matrix()
+    m = O.make_matrix() if matrix is None else matrix
     params = O.Params()
     per_ref = []
     for name in names:

@@ -15,7 +15,7 @@ sys.path.insert(0, HERE)
 sys.path.insert(0, ROOT)
 
 import golden_util as G  # noqa: E402
-from test_cli_dropin import _info_stats, _snapshot  # noqa: E402
+from test_cli_dropin import SCORING_ARGS, _info_stats, _snapshot  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
@@ -34,7 +34,8 @@ def _fastq(tmp_path, case):
 
 @pytest.mark.parametrize("case,extra", [("fanc_cas9", ["--write_detailed_allele_table"]),
                                         ("synth_hdr", []),
-                                        ("synth_single", ["--ignore_substitutions", "-w", "10"])])
+                                        ("synth_single", ["--ignore_substitutions", "-w", "10"]),
+                                        ("fanc_cas9", SCORING_ARGS)])
 def test_launcher_output_folder_equals_the_reference(case, extra, tmp_path):
     from baseline import ref_shim
     if not ref_shim.available():

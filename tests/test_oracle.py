@@ -107,12 +107,15 @@ def test_whole_path_golden(case, ednafull):
 
 # ---- fuzz against the compiled reference (its answers recorded: tests/reference_record.py) -------------------
 REC = reference_record.Record("reference_oracle_fuzz")
+SREC = reference_record.Record("reference_scoring_fuzz")
+MATRIX_FILE = os.path.join(G.GOLD, "scoring_nuc.matrix")
 
 
 @pytest.fixture(scope="module", autouse=True)
 def _save_records():
     yield
     REC.save()
+    SREC.save()
 
 
 def test_live_fuzz_against_compiled_reference(ednafull):
@@ -138,6 +141,91 @@ def test_live_fuzz_against_compiled_reference(ednafull):
                                                    for k, v in mods[1].find_indels_substitutions(want[0], want[1], inc).__dict__.items()})
         g = O.find_indels_substitutions(want[0], want[1], inc)
         assert not G.payload_equal(w, g)
+
+
+def test_matrix_file_against_compiled_reference():
+    """The NCBI-format fixture tests/golden/scoring_nuc.matrix (asymmetric, N-N above every match) read by oracle.read_matrix
+    and by the reference's own read_matrix."""
+    mods = O.ref_modules() if reference_record.RECORDING else None
+    want = SREC.value("read_matrix", lambda: np.asarray(mods[0].read_matrix(MATRIX_FILE)))
+    got = O.read_matrix(MATRIX_FILE)
+    assert got.shape == want.shape and (got == want).all()
+    assert got[ord("A"), ord("C")] != got[ord("C"), ord("A")] and got[ord("N"), ord("N")] > got[ord("G"), ord("G")]
+
+
+def scoring_case(rng, k, ednafull):
+    """Case k of the scoring-space fuzz -> (read, ref, matrix, gap_incentive, gap_open, gap_extend, label).  Matrices: make_matrix
+    with varied scores (mismatch >= 0 and N-N above the match score included), asymmetric tables, the NCBI-format fixture, and
+    EDNAFULL scaled by 2^16 .. 2^21 (I, J <= 150, where the reference's int32 DP is still exact).  Gap pairs include go == ge,
+    go > ge, ge = 0, go = ge = 0 and positive values (only the drop-in global_align receives those).  Incentives: zero,
+    cut-only, non-zero gi[0] and gi[I], dense random and negative."""
+    kind = k % 5
+    if kind == 0:
+        m = O.make_matrix(rng.randint(1, 12), rng.randint(-12, 2), rng.randint(-6, 3), rng.randint(-3, 14))
+    elif kind == 1:
+        m = np.array(ednafull, dtype=np.int64)
+        for a in "ACGTN":
+            for b in "ACGTN":
+                if rng.random() < 0.4:
+                    m[ord(a), ord(b)] += rng.randint(-4, 4)
+    elif kind == 2:
+        m = O.read_matrix(MATRIX_FILE)
+    elif kind == 3:
+        m = np.array(ednafull, dtype=np.int64) << rng.randint(16, 21)
+    else:
+        m = np.array(ednafull, dtype=np.int64)
+    I = rng.choice([5, 12, 40, 90, 150])
+    ref = "".join(rng.choice("ACGT" if rng.random() < 0.8 else "ACGTN") for _ in range(I))
+    read = "".join(c if rng.random() > 0.1 else rng.choice("ACGTN") for c in ref)
+    cut = rng.randrange(I)
+    u = rng.random()
+    if u < 0.4:
+        read = read[:cut] + read[cut + rng.randrange(1, 8):]
+    elif u < 0.7:
+        read = read[:cut] + "".join(rng.choice("ACGT") for _ in range(rng.randrange(1, 8))) + read[cut:]
+    read = read[:150] or "A"
+    go, ge = rng.choice([(-20, -2), (-5, -5), (-1, -5), (-10, 0), (-3, -1), (0, 0), (2, 1), (-2, 3)])
+    gi = Z(I + 1)
+    prof = rng.randrange(5)
+    if prof == 1:
+        gi[cut + 1] = rng.randint(1, 6)
+    elif prof == 2:
+        gi[0], gi[I], gi[cut + 1] = rng.randint(1, 5), rng.randint(1, 5), 1
+    elif prof == 3:
+        gi[:] = [rng.randint(0, 3) for _ in range(I + 1)]
+    elif prof == 4:
+        gi[cut + 1] = -rng.randint(1, 6)
+        gi[rng.randrange(I + 1)] -= rng.randint(0, 3)
+    if kind == 3 and rng.random() < 0.5:
+        gi *= 1 << rng.randint(10, 18)
+    return read, ref, np.ascontiguousarray(m), gi, go, ge, "m%d gi%d" % (kind, prof)
+
+
+def test_scoring_fuzz_against_compiled_reference(ednafull):
+    """The oracle beyond EDNAFULL: global_align and find_indels_substitutions of the compiled reference (answers recorded in
+    tests/golden/reference_scoring_fuzz.json.gz) over matrices, gap pairs, incentive profiles and magnitudes.  Cases where
+    the reference's traceback reads a pointer it never set (the oracle's rc = -3) are recorded as such."""
+    mods = O.ref_modules() if reference_record.RECORDING else None
+    rng = random.Random(11)
+    undefined, kinds = 0, set()
+    for k in range(360):
+        read, ref, m, gi, go, ge, label = scoring_case(rng, k, ednafull)
+        try:
+            got = O.global_align(read, ref, m, gi, go, ge)
+        except O.OracleUndefined:
+            got = "undefined"
+        want = SREC.value("align %d" % k, lambda: "undefined" if got == "undefined" else
+                          tuple(mods[0].global_align(read, ref, matrix=m, gap_incentive=gi, gap_open=go, gap_extend=ge)))
+        assert got == want, (k, label, go, ge)
+        if got == "undefined":
+            undefined += 1
+            continue
+        kinds.add(label)
+        inc = sorted(rng.sample(range(len(ref)), min(len(ref), 4)))
+        w = SREC.value("payload %d" % k, lambda: {key: (v.tolist() if hasattr(v, "tolist") else v)
+                                                  for key, v in mods[1].find_indels_substitutions(want[0], want[1], inc).__dict__.items()})
+        assert not G.payload_equal(w, O.find_indels_substitutions(want[0], want[1], inc)), (k, label)
+    assert len(kinds) == 25 and undefined < 60, (sorted(kinds), undefined)
 
 
 def test_legacy_classification_restatement_against_compiled_reference():
