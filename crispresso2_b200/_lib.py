@@ -27,6 +27,7 @@ F_NO_PAIRING = 128
 F_HDR_REF1 = 256
 F_NO_RING = 512
 F_LEGACY_INS = 1024
+ANN_SAM_OPTIONAL = 1 << 16                              # C2B_ANN_SAM_OPTIONAL: c2b_annotate_build's process_bam form
 
 ST_BAD_CHAR = 1
 ST_UNDEFINED = 2
@@ -82,7 +83,7 @@ EXPORTS = ["c2b_create", "c2b_destroy", "c2b_last_error", "c2b_configure", "c2b_
            "c2b_align_batch_device", "c2b_set_pair_order", "c2b_sync", "c2b_stream", "c2b_last_kernel_ms", "c2b_launch_count", "c2b_path_counts", "c2b_band_reruns", "c2b_ring_counts", "c2b_diag_counts",
            "c2b_counts_layout", "c2b_counts_hist_layout", "c2b_counts_reset", "c2b_counts_read", "c2b_counts_device", "c2b_global_align",
            "c2b_classify_aligned", "c2b_classify_aligned_flags", "c2b_host_alloc", "c2b_host_free",
-           "c2b_fastq_dedup", "c2b_fastq_dedup_buffer", "c2b_fastq_gpu_available", "c2b_fastq_dedup_gpu", "c2b_fastq_dedup_gpu_buffer", "c2b_fastq_n_reads", "c2b_fastq_n_unique", "c2b_fastq_max_len",
+           "c2b_fastq_dedup", "c2b_fastq_dedup_buffer", "c2b_fastq_gpu_available", "c2b_fastq_dedup_gpu", "c2b_fastq_dedup_gpu_buffer", "c2b_sam_dedup_gpu_buffer", "c2b_sam_dedup_buffer", "c2b_fastq_n_reads", "c2b_fastq_n_unique", "c2b_fastq_max_len",
            "c2b_fastq_seqs", "c2b_fastq_offsets", "c2b_fastq_counts", "c2b_fastq_first_index", "c2b_fastq_free",
            "c2b_fastq_last_error", "c2b_fastq_filter", "c2b_fastq_filter_pair", "c2b_rc_merge_weights", "c2b_screen_reads", "c2b_serial_stats",
            "c2b_consensus_from_pairs", "c2b_alleles_build", "c2b_alleles_free", "c2b_alleles_n", "c2b_alleles_order", "c2b_alleles_arena", "c2b_alleles_offsets",
@@ -90,7 +91,7 @@ EXPORTS = ["c2b_create", "c2b_destroy", "c2b_last_error", "c2b_configure", "c2b_
            "c2b_annotate_build", "c2b_annotate_free", "c2b_annotate_n", "c2b_annotate_arena", "c2b_annotate_offsets",
            "c2b_annotate_cigar_arena", "c2b_annotate_cigar_offsets", "c2b_annotate_flags", "c2b_annotate_mapq", "c2b_annotate_first",
            "c2b_annotate_last_record", "c2b_annotate_record_arena", "c2b_annotate_record_offsets", "c2b_annotate_write_fastq",
-           "c2b_annotate_write_sam"]
+           "c2b_annotate_write_sam", "c2b_annotate_write_sam_passthrough"]
 
 _cache = {}
 
@@ -197,6 +198,10 @@ def load(path=None):
     L.c2b_fastq_dedup_gpu.argtypes = [C.c_char_p, i32, C.POINTER(vp)]
     L.c2b_fastq_dedup_gpu_buffer.restype = C.c_int
     L.c2b_fastq_dedup_gpu_buffer.argtypes = [vp, C.c_size_t, i32, C.POINTER(vp)]
+    L.c2b_sam_dedup_gpu_buffer.restype = C.c_int
+    L.c2b_sam_dedup_gpu_buffer.argtypes = [vp, C.c_size_t, i32, C.POINTER(vp)]
+    L.c2b_sam_dedup_buffer.restype = C.c_int
+    L.c2b_sam_dedup_buffer.argtypes = [vp, C.c_size_t, i32, C.POINTER(vp)]
     L.c2b_fastq_filter.restype = C.c_int
     L.c2b_fastq_filter.argtypes = [C.c_char_p, C.c_char_p, i32, i32, i32, i32, C.POINTER(i64), C.POINTER(i64)]
     L.c2b_fastq_filter_pair.restype = C.c_int
@@ -244,5 +249,7 @@ def load(path=None):
     L.c2b_annotate_write_fastq.argtypes = [vp, vp, vp, i64, C.c_char_p, C.c_char_p, i32]
     L.c2b_annotate_write_sam.restype = C.c_int
     L.c2b_annotate_write_sam.argtypes = [vp, vp, vp, i64, C.c_char_p, C.c_char_p, C.c_char_p, i32, cpp, cpp, vp, i32]
+    L.c2b_annotate_write_sam_passthrough.restype = C.c_int
+    L.c2b_annotate_write_sam_passthrough.argtypes = [vp, vp, vp, i64, vp, C.c_size_t, C.c_char_p, i32]
     _cache[path] = L
     return L

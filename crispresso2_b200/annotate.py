@@ -65,7 +65,8 @@ def _cstrings(items):
 class Annotation:
     """Per-unique-read annotations of the process_fastq call that filled `variantCache` (one GPU pass, host arena)."""
 
-    def __init__(self, variantCache, refs, sam_strands=False, chunk=0):
+    def __init__(self, variantCache, refs, sam_strands=False, chunk=0, sam_optional=False):
+        """sam_optional: the text of process_bam (C2B_ANN_SAM_OPTIONAL): "c2:Z:" first, no scores / details for aligned reads"""
         src = core.source_of(variantCache)
         if len(src.parts) != 1:
             raise NotImplementedError("annotated outputs of a run sharded over several processes are not built")
@@ -133,7 +134,8 @@ class Annotation:
                                   R, NW, edits.shape[2], recs.ctypes.data, alns.ctypes.data, ops.ctypes.data, meta.ctypes.data,
                                   edits.ctypes.data, amask.ctypes.data, aname.ctypes.data, label.ctypes.data,
                                   len(names), _cstrings(names), rev.ctypes.data, len(labels), _cstrings(labels),
-                                  _cstrings(seqs), lens.ctypes.data, comp.ctypes.data, flags & _lib.F_LEGACY_INS, int(chunk), C.byref(h))
+                                  _cstrings(seqs), lens.ctypes.data, comp.ctypes.data,
+                                  (flags & _lib.F_LEGACY_INS) | (_lib.ANN_SAM_OPTIONAL if sam_optional else 0), int(chunk), C.byref(h))
         if rc != 0:
             raise core.EngineError("c2b_annotate_build failed (%d): %s" % (rc, L.c2b_last_error(eng.h).decode()))
         self.h = h
@@ -154,7 +156,7 @@ class Annotation:
             self.L.c2b_annotate_free(h)
 
     def text(self, u):
-        """annotation of unique read u (the FASTQ form: leading space)"""
+        """annotation of unique read u (the FASTQ form: leading space; the process_bam form: "c2:Z:" first)"""
         return self.arena[self.ann_off[u]:self.ann_off[u + 1]].tobytes().decode("ascii")
 
     # ---------------------------------------------------------------------------------------------------- writers
@@ -190,6 +192,17 @@ class Annotation:
         self.mapq = self._view("c2b_annotate_mapq", C.c_int32, self.n)
         self.first = first
 
+    def write_sam_passthrough(self, text, sam_out):
+        """pass 2 of process_bam: the lines of `text` (SAM, bytes) whose read is a unique read here, with their annotation,
+        appended to sam_out"""
+        arr = np.frombuffer(text, dtype=np.uint8)
+        rc = self.L.c2b_annotate_write_sam_passthrough(self.h, self.buf.ctypes.data if len(self.buf) else None, self.off.ctypes.data,
+                                                       self.n, arr.ctypes.data if len(arr) else None, len(arr), os.fsencode(sam_out), 0)
+        if rc == _lib.E_LIMIT:
+            raise IndexError("list index out of range: %s" % self.L.c2b_fastq_last_error().decode())
+        if rc != 0:
+            raise core.EngineError("c2b_annotate_write_sam_passthrough failed (%d): %s" % (rc, self.L.c2b_fastq_last_error().decode()))
+
     # ---------------------------------------------------------------------------------------------------- cache entries
     def annotation_of(self, k):
         """'crispresso2_annotation' of batch read k (aligned reads only, CRISPRessoCORE.py:2343)"""
@@ -213,12 +226,13 @@ class Annotation:
                 self.cig[self.cig_off[u]:self.cig_off[u + 1]].tobytes().decode("ascii"), "*", "0", "0", seq, qual,
                 "c2:Z:" + self.text(u)[1:]]
 
-    def attach(self, variantCache, key, value_of):
-        """variantCache entries get `key` when they materialise; entries already materialised get it now"""
+    def attach(self, variantCache, key, value_of, also=()):
+        """variantCache entries (and those of the dicts in `also`, filled by the same call: not_aligned_variants) get `key` when
+        they materialise; entries already materialised get it now"""
         src = self.src
         src.extra_keys.append((key, value_of))
         if src.n_filled:
-            for v in variantCache.values():
+            for v in (v for d in (variantCache,) + tuple(also) for v in d.values()):
                 k = getattr(v, "_k", -1)
                 if k < -1:
                     val = value_of(-2 - k)

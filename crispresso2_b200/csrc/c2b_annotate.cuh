@@ -92,9 +92,11 @@ C2B_DEV int lane_excl_scan(int v)
 // Aligned read (which = 0) or reference (which = 1) string of one slot, left to right, n columns (Align.pyx:422-432):
 // column q from the right consumes read / reference when its op is not a gap on that side; the idx-th consuming column from
 // the right holds read[rlen - 1 - idx] (forward strand), comp[read[idx]] (reverse complement) or ref[ilen - 1 - idx].
+// Only columns [lo, hi) counted from the left are written (hi < 0: all n).
 C2B_DEV void spell(Out &o, const uint64_t *ops, int n, int which, const uint8_t *read, int rlen, int strand, const char *ref,
-                   int ilen, const uint8_t *comp)
+                   int ilen, const uint8_t *comp, int lo = 0, int hi = -1)
 {
+    if (hi < 0) hi = n;
     const int l = wp::lane();
     const uint64_t w = (32 * l < n) ? ops[l] : 0ull;
     const int gap = which ? OP_I : OP_J;
@@ -109,9 +111,10 @@ C2B_DEV void spell(Out &o, const uint64_t *ops, int n, int which, const uint8_t 
                 c = which ? ref[ilen - 1 - idx] : strand ? (char)comp[read[idx]] : (char)read[rlen - 1 - idx];
                 idx++;
             }
-            o.p[o.n + (n - 1 - q)] = c;
+            const int col = n - 1 - q;
+            if (col >= lo && col < hi) o.p[o.n + (col - lo)] = c;
         }
-    o.n += n;
+    o.n += hi - lo;
 }
 
 // ref_positions.index(a) (COREResources.pyx:105-133): the column, from the left, that holds reference base a; -1 if none
@@ -161,15 +164,27 @@ C2B_DEV void put_copy(Out &o, int64_t from, int n)
     o.n += n;
 }
 
-// one unique read: annotation text (+ CIGAR / flag / MAPQ of the first listed slot)
+// columns [lo, hi) of slot s's aligned read (which = 0) or reference (which = 1)
+C2B_DEV void spell_slot(Out &o, const AParams &P, int64_t k, int s, int which, const uint8_t *read, int rlen, int lo, int hi)
+{
+    const int R = P.R;
+    spell(o, P.ops + (k * R + s) * P.NW, slot_cols(P, k, s), which, read, rlen, (int)((P.meta[k * R + s] >> 16) & 1u),
+          P.refseq + P.ref_off[s], P.ref_off[s + 1] - P.ref_off[s], P.comp, lo, hi);
+}
+
+// one unique read: annotation text (+ CIGAR / flag / MAPQ of the first listed slot).  With C2B_ANN_SAM_OPTIONAL (process_bam,
+// CRISPRessoCORE.py:2217-2234) the text starts with "c2:Z:" instead of a space and an aligned read has no ALN_SCORES /
+// ALN_DETAILS: its INS bases, ALN_REF and ALN_SEQ are spelled from the op stream instead of copied from the details.
 template <bool WRITE>
 C2B_DEV void annotate_one(const AParams &P, int64_t u)
 {
     Out o{WRITE ? P.ann + P.ann_off[u] : nullptr, 0};
     const int64_t k = P.bidx[u];
-    const char *na = " ALN=NA";
+    const bool samf = (P.flags & C2B_ANN_SAM_OPTIONAL) != 0;
+    const char *na = samf ? "c2:Z:ALN=NA" : " ALN=NA";
+    const int nna = samf ? 11 : 7;
     if (k < 0) {                                                // outside the engine's contract: no scores, no details
-        put_str(o, na, 7);
+        put_str(o, na, nna);
         put_str(o, " ALN_SCORES= ALN_DETAILS=", 25);
         if (!WRITE) { if (wp::lane() == 0) { P.ann_len[u] = o.n; P.cig_len[u] = 0; } }
         else if (wp::lane() == 0) { P.flag[u] = 255; P.mapq[u] = 0; P.first[u] = -1; }
@@ -180,30 +195,32 @@ C2B_DEV void annotate_one(const AParams &P, int64_t u)
     const int rlen = (int)(P.roff[u + 1] - P.roff[u]);
     int slot[32], name[32];
     const int nl = listed(P, k, slot, name);
-    if (nl == 0) put_str(o, na, 7);
+    if (nl == 0) put_str(o, na, nna);
     else {
-        put_str(o, " ALN=", 5);
+        if (samf) put_str(o, "c2:Z:ALN=", 9); else put_str(o, " ALN=", 5);
         for (int x = 0; x < nl; x++) { if (x) put(o, '&'); put_name(o, P, name[x]); }
     }
-    put_str(o, " ALN_SCORES=", 12);
-    for (int r = 0; r < R; r++) { if (r) put(o, '&'); put_score(o, P.alns[k * R + r].score_milli); }
-    put_str(o, " ALN_DETAILS=", 13);
     int64_t det[32];                                            // where slot r's aligned read starts in this annotation
-    for (int r = 0; r < R; r++) {
-        if (r) put(o, '&');
-        put_name(o, P, r);
-        put(o, ',');
-        const int n = slot_cols(P, k, r);
-        const int strand = (int)((P.meta[k * R + r] >> 16) & 1u);
-        const uint64_t *ops = P.ops + (k * R + r) * P.NW;
-        const char *ref = P.refseq + P.ref_off[r];
-        const int ilen = P.ref_off[r + 1] - P.ref_off[r];
-        det[r] = o.n;
-        spell(o, ops, n, 0, read, rlen, strand, ref, ilen, P.comp);
-        put(o, ',');
-        spell(o, ops, n, 1, read, rlen, strand, ref, ilen, P.comp);
-        put(o, ',');
-        put_score(o, P.alns[k * R + r].score_milli);
+    if (!samf || nl == 0) {                                     // the process_bam form lists them for not-aligned reads only
+        put_str(o, " ALN_SCORES=", 12);
+        for (int r = 0; r < R; r++) { if (r) put(o, '&'); put_score(o, P.alns[k * R + r].score_milli); }
+        put_str(o, " ALN_DETAILS=", 13);
+        for (int r = 0; r < R; r++) {
+            if (r) put(o, '&');
+            put_name(o, P, r);
+            put(o, ',');
+            const int n = slot_cols(P, k, r);
+            const int strand = (int)((P.meta[k * R + r] >> 16) & 1u);
+            const uint64_t *ops = P.ops + (k * R + r) * P.NW;
+            const char *ref = P.refseq + P.ref_off[r];
+            const int ilen = P.ref_off[r + 1] - P.ref_off[r];
+            det[r] = o.n;
+            spell(o, ops, n, 0, read, rlen, strand, ref, ilen, P.comp);
+            put(o, ',');
+            spell(o, ops, n, 1, read, rlen, strand, ref, ilen, P.comp);
+            put(o, ',');
+            put_score(o, P.alns[k * R + r].score_milli);
+        }
     }
     wp::sync();                                                 // the spelled strings are read back below
     if (nl) {
@@ -252,16 +269,27 @@ C2B_DEV void annotate_one(const AParams &P, int64_t u)
                         const int ilen = P.ref_off[s + 1] - P.ref_off[s];
                         const int c = ref_column(P.ops + (k * R + s) * P.NW, n, ilen, E.a);
                         const int lo = c + 1, hi = lo + (int)E.b < n ? lo + (int)E.b : n;
-                        if (hi > lo) put_copy(o, det[s] + lo, hi - lo);
+                        if (hi > lo) {
+                            if (samf) spell_slot(o, P, k, s, 0, read, rlen, lo, hi);
+                            else put_copy(o, det[s] + lo, hi - lo);
+                        }
                     }
                     put(o, ')');
                 }
             }
         }
         put_str(o, " ALN_REF=", 9);
-        for (int x = 0; x < nl; x++) { if (x) put(o, '&'); const int n = slot_cols(P, k, slot[x]); put_copy(o, det[slot[x]] + n + 1, n); }
+        for (int x = 0; x < nl; x++) {
+            if (x) put(o, '&');
+            const int n = slot_cols(P, k, slot[x]);
+            if (samf) spell_slot(o, P, k, slot[x], 1, read, rlen, 0, n); else put_copy(o, det[slot[x]] + n + 1, n);
+        }
         put_str(o, " ALN_SEQ=", 9);
-        for (int x = 0; x < nl; x++) { if (x) put(o, '&'); put_copy(o, det[slot[x]], slot_cols(P, k, slot[x])); }
+        for (int x = 0; x < nl; x++) {
+            if (x) put(o, '&');
+            const int n = slot_cols(P, k, slot[x]);
+            if (samf) spell_slot(o, P, k, slot[x], 0, read, rlen, 0, n); else put_copy(o, det[slot[x]], n);
+        }
     }
     // CIGAR of the first listed slot: runs of M / I (gap in the reference) / D (gap in the read) from the left; elements in
     // reverse order when refs[first]['aln_strand'] == '-' (CRISPRessoCORE.py:2462-2467)

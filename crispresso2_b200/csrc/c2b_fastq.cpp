@@ -96,11 +96,13 @@ bool read_plain(const char *path, c2b_bytes &buf, std::string &err)
 }
 
 // output parts written at their offsets by all host threads
-bool write_parts(const char *path, const std::vector<std::string> &parts, const std::string &tail)
+// (append: after the file's current end)
+bool write_parts(const char *path, const std::vector<std::string> &parts, const std::string &tail, bool append = false)
 {
-    int fd = open(path, O_WRONLY | O_CREAT | O_TRUNC, 0666);
+    int fd = open(path, O_WRONLY | O_CREAT | (append ? 0 : O_TRUNC), 0666);
     if (fd < 0) return false;
     std::vector<size_t> off(parts.size() + 1, 0);
+    if (append) { const off_t end = lseek(fd, 0, SEEK_END); if (end < 0) { close(fd); return false; } off[0] = (size_t)end; }
     for (size_t k = 0; k < parts.size(); k++) off[k + 1] = off[k] + parts[k].size();
     const size_t total = off[parts.size()] + tail.size();
     if (total && ftruncate(fd, (off_t)total) != 0) { close(fd); return false; }
@@ -218,12 +220,106 @@ bool read_gz(const char *path, c2b_bytes &buf, std::string &err)
     return true;
 }
 
+// (3) sharded exact dedup in file order and (4) the unique reads in first-seen order, from every record's sequence and hash:
+// shared by the FASTQ front end and the SAM one (c2b_sam_dedup_buffer)
+void dedup_records(const std::vector<Seq> &seq, const std::vector<uint64_t> &hv, int64_t n_rec, int T, c2b_fastq *F,
+                   const std::function<void(const char *)> &lap)
+{
+    // (3) sharded exact dedup in file order
+    struct Ent { int64_t first; int32_t count; };
+    std::vector<std::vector<Ent>> found(T);
+    auto shard = [&](int s) {
+        size_t mine = 0;
+        for (int64_t r = 0; r < n_rec; r++) mine += ((hv[(size_t)r] >> 40) % (uint64_t)T) == (uint64_t)s;
+        size_t cap = 64;
+        while (cap < mine * 2 + 8) cap <<= 1;
+        std::vector<int32_t> slot(cap, -1);                // index into found[s]
+        auto &E = found[s];
+        for (int64_t r = 0; r < n_rec; r++) {
+            const uint64_t h = hv[(size_t)r];
+            if (((h >> 40) % (uint64_t)T) != (uint64_t)s) continue;
+            size_t k = (size_t)h & (cap - 1);
+            for (;;) {
+                const int32_t e = slot[k];
+                if (e < 0) { slot[k] = (int32_t)E.size(); E.push_back({r, 1}); break; }
+                const Seq &a = seq[(size_t)E[(size_t)e].first], &b = seq[(size_t)r];
+                if (hv[(size_t)E[(size_t)e].first] == h && a.len == b.len && memcmp(a.p, b.p, a.len) == 0) { E[(size_t)e].count++; break; }
+                k = (k + 1) & (cap - 1);
+            }
+        }
+    };
+    {
+        std::vector<std::thread> th;
+        for (int t = 1; t < T; t++) th.emplace_back(shard, t);
+        shard(0);
+        for (auto &x : th) x.join();
+    }
+
+    lap("dedup");
+    // (4) unique reads in first-seen order: the shards' entries are scattered to their first record (disjoint records, so
+    // in parallel), a prefix count over the records numbers them -- no sort, no serial pass over the unique reads
+    std::vector<int32_t> cnt_at((size_t)n_rec, 0);
+    {
+        auto scatter = [&](int t) { for (const Ent &e : found[(size_t)t]) cnt_at[(size_t)e.first] = e.count; };
+        std::vector<std::thread> th;
+        for (int t = 1; t < T; t++) th.emplace_back(scatter, t);
+        scatter(0);
+        for (auto &x : th) x.join();
+    }
+    std::vector<size_t> u0((size_t)T + 1, 0);              // unique reads / bytes before thread t's record range
+    std::vector<int64_t> b0((size_t)T + 1, 0);
+    std::vector<int32_t> mx((size_t)T, 0);
+    auto rec_lo = [&](int t) { return n_rec * t / T; };
+    {
+        auto count = [&](int t) {
+            size_t u = 0; int64_t by = 0; int32_t m = 0;
+            for (int64_t r = rec_lo(t); r < rec_lo(t + 1); r++) if (cnt_at[(size_t)r]) { u++; by += seq[(size_t)r].len; m = std::max<int32_t>(m, (int32_t)seq[(size_t)r].len); }
+            u0[(size_t)t + 1] = u; b0[(size_t)t + 1] = by; mx[(size_t)t] = m;
+        };
+        std::vector<std::thread> th;
+        for (int t = 1; t < T; t++) th.emplace_back(count, t);
+        count(0);
+        for (auto &x : th) x.join();
+    }
+    for (int t = 0; t < T; t++) { u0[(size_t)t + 1] += u0[(size_t)t]; b0[(size_t)t + 1] += b0[(size_t)t]; F->max_len = std::max(F->max_len, mx[(size_t)t]); }
+    const size_t nu = u0[(size_t)T];
+    const int64_t tot = b0[(size_t)T];
+    F->offsets.resize(nu + 1);
+    F->counts.resize(nu);
+    F->first_index.resize(nu);
+    F->offsets[nu] = tot;
+    F->seqs.reset(new uint8_t[(size_t)tot + 16]);
+    {
+        auto emit = [&](int t) {
+            size_t u = u0[(size_t)t]; int64_t by = b0[(size_t)t];
+            for (int64_t r = rec_lo(t); r < rec_lo(t + 1); r++) {
+                const int32_t c = cnt_at[(size_t)r];
+                if (!c) continue;
+                const Seq &q = seq[(size_t)r];
+                F->offsets[u] = by; F->counts[u] = c; F->first_index[u] = r;
+                memcpy(F->seqs.get() + by, q.p, q.len);
+                by += q.len; u++;
+            }
+        };
+        std::vector<std::thread> th;
+        for (int t = 1; t < T; t++) th.emplace_back(emit, t);
+        emit(0);
+        for (auto &x : th) x.join();
+    }
+    lap("emit");
+}
+
 }  // namespace
 
 static std::string g_fastq_err;
 
 bool c2b_fastq_read_gz(const char *path, c2b_bytes &buf, std::string &err) { return read_gz(path, buf, err); }
 void c2b_fastq_set_error(const std::string &m) { g_fastq_err = m; }
+int c2b_sam_line_error(int64_t line, int kind)
+{
+    g_fastq_err = "SAM text line " + std::to_string(line + 1) + (kind ? ": fewer than 10 tab-separated fields" : ": non-ASCII byte (out of contract)");
+    return kind ? C2B_E_LIMIT : C2B_E_ARG;
+}
 
 extern "C" {
 
@@ -319,88 +415,7 @@ int c2b_fastq_dedup_buffer(const uint8_t *data, size_t n, int32_t n_threads, c2b
     }
 
     lap("hash");
-    // (3) sharded exact dedup in file order
-    struct Ent { int64_t first; int32_t count; };
-    std::vector<std::vector<Ent>> found(T);
-    auto shard = [&](int s) {
-        size_t mine = 0;
-        for (int64_t r = 0; r < n_rec; r++) mine += ((hv[(size_t)r] >> 40) % (uint64_t)T) == (uint64_t)s;
-        size_t cap = 64;
-        while (cap < mine * 2 + 8) cap <<= 1;
-        std::vector<int32_t> slot(cap, -1);                // index into found[s]
-        auto &E = found[s];
-        for (int64_t r = 0; r < n_rec; r++) {
-            const uint64_t h = hv[(size_t)r];
-            if (((h >> 40) % (uint64_t)T) != (uint64_t)s) continue;
-            size_t k = (size_t)h & (cap - 1);
-            for (;;) {
-                const int32_t e = slot[k];
-                if (e < 0) { slot[k] = (int32_t)E.size(); E.push_back({r, 1}); break; }
-                const Seq &a = seq[(size_t)E[(size_t)e].first], &b = seq[(size_t)r];
-                if (hv[(size_t)E[(size_t)e].first] == h && a.len == b.len && memcmp(a.p, b.p, a.len) == 0) { E[(size_t)e].count++; break; }
-                k = (k + 1) & (cap - 1);
-            }
-        }
-    };
-    {
-        std::vector<std::thread> th;
-        for (int t = 1; t < T; t++) th.emplace_back(shard, t);
-        shard(0);
-        for (auto &x : th) x.join();
-    }
-
-    lap("dedup");
-    // (4) unique reads in first-seen order: the shards' entries are scattered to their first record (disjoint records, so
-    // in parallel), a prefix count over the records numbers them -- no sort, no serial pass over the unique reads
-    std::vector<int32_t> cnt_at((size_t)n_rec, 0);
-    {
-        auto scatter = [&](int t) { for (const Ent &e : found[(size_t)t]) cnt_at[(size_t)e.first] = e.count; };
-        std::vector<std::thread> th;
-        for (int t = 1; t < T; t++) th.emplace_back(scatter, t);
-        scatter(0);
-        for (auto &x : th) x.join();
-    }
-    std::vector<size_t> u0((size_t)T + 1, 0);              // unique reads / bytes before thread t's record range
-    std::vector<int64_t> b0((size_t)T + 1, 0);
-    std::vector<int32_t> mx((size_t)T, 0);
-    auto rec_lo = [&](int t) { return n_rec * t / T; };
-    {
-        auto count = [&](int t) {
-            size_t u = 0; int64_t by = 0; int32_t m = 0;
-            for (int64_t r = rec_lo(t); r < rec_lo(t + 1); r++) if (cnt_at[(size_t)r]) { u++; by += seq[(size_t)r].len; m = std::max<int32_t>(m, (int32_t)seq[(size_t)r].len); }
-            u0[(size_t)t + 1] = u; b0[(size_t)t + 1] = by; mx[(size_t)t] = m;
-        };
-        std::vector<std::thread> th;
-        for (int t = 1; t < T; t++) th.emplace_back(count, t);
-        count(0);
-        for (auto &x : th) x.join();
-    }
-    for (int t = 0; t < T; t++) { u0[(size_t)t + 1] += u0[(size_t)t]; b0[(size_t)t + 1] += b0[(size_t)t]; F->max_len = std::max(F->max_len, mx[(size_t)t]); }
-    const size_t nu = u0[(size_t)T];
-    const int64_t tot = b0[(size_t)T];
-    F->offsets.resize(nu + 1);
-    F->counts.resize(nu);
-    F->first_index.resize(nu);
-    F->offsets[nu] = tot;
-    F->seqs.reset(new uint8_t[(size_t)tot + 16]);
-    {
-        auto emit = [&](int t) {
-            size_t u = u0[(size_t)t]; int64_t by = b0[(size_t)t];
-            for (int64_t r = rec_lo(t); r < rec_lo(t + 1); r++) {
-                const int32_t c = cnt_at[(size_t)r];
-                if (!c) continue;
-                const Seq &q = seq[(size_t)r];
-                F->offsets[u] = by; F->counts[u] = c; F->first_index[u] = r;
-                memcpy(F->seqs.get() + by, q.p, q.len);
-                by += q.len; u++;
-            }
-        };
-        std::vector<std::thread> th;
-        for (int t = 1; t < T; t++) th.emplace_back(emit, t);
-        emit(0);
-        for (auto &x : th) x.join();
-    }
-    lap("emit");
+    dedup_records(seq, hv, n_rec, T, F, lap);
     *out = F;
     return C2B_OK;
 }
@@ -440,6 +455,7 @@ int c2b_fastq_dedup(const char *path, int32_t n_threads, c2b_fastq **out)
 int c2b_fastq_gpu_available(void) { return 0; }
 int c2b_fastq_dedup_gpu(const char *, int32_t, c2b_fastq **out) { if (out) *out = nullptr; g_fastq_err = "c2b_fastq_dedup_gpu: not built (emulator)"; return C2B_E_STATE; }
 int c2b_fastq_dedup_gpu_buffer(const uint8_t *, size_t, int32_t, c2b_fastq **out) { if (out) *out = nullptr; g_fastq_err = "c2b_fastq_dedup_gpu: not built (emulator)"; return C2B_E_STATE; }
+int c2b_sam_dedup_gpu_buffer(const uint8_t *, size_t, int32_t, c2b_fastq **out) { if (out) *out = nullptr; g_fastq_err = "c2b_sam_dedup_gpu_buffer: not built (emulator)"; return C2B_E_STATE; }
 #endif
 
 int64_t c2b_fastq_n_reads(const c2b_fastq *f) { return f ? f->n_reads : 0; }
@@ -1091,6 +1107,123 @@ extern "C" int c2b_annotate_write_sam(c2b_annotation *a, const uint8_t *seqs, co
             a->rec.append((const char *)ql.p, ql.len);
         } else a->rec_off.push_back((int64_t)a->rec.size());
         a->rec_off.push_back((int64_t)a->rec.size());
+    }
+    return C2B_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ SAM text (process_bam)
+// Replaces the two `samtools view` loops of process_bam (CRISPRessoCORE.py:2047-2057 and :2251-2262), whose lines are read in
+// text mode (universal newlines) and split as line.rstrip().split("\t"): the read is field 10.
+namespace {
+
+// field 10 of line.rstrip().split("\t"): [s0, s1) within the line, e = the rstrip end; false when there are fewer than 10 fields
+bool sam_field10(const uint8_t *p, uint32_t len, uint32_t &s0, uint32_t &s1, uint32_t &e)
+{
+    e = len;
+    while (e && is_space(p[e - 1])) e--;
+    uint32_t i = 0;
+    for (int tabs = 0; tabs < 9; tabs++) {
+        const uint8_t *q = (const uint8_t *)memchr(p + i, '\t', e - i);
+        if (!q) return false;
+        i = (uint32_t)(q - p) + 1;
+    }
+    s0 = i;
+    const uint8_t *q = (const uint8_t *)memchr(p + i, '\t', e - i);
+    s1 = q ? (uint32_t)(q - p) : e;
+    return true;
+}
+
+// the first bad line of lines [lo, hi) as (line << 1) | kind (kind 0: a non-ASCII byte, 1: fewer than 10 fields), or -1
+int64_t sam_first_bad(const uint8_t *data, const std::vector<TLine> &lines, size_t lo, size_t hi)
+{
+    for (size_t k = lo; k < hi; k++) {
+        const uint8_t *p = data + lines[k].p;
+        for (uint32_t i = 0; i < lines[k].len; i++) if (p[i] & 0x80) return (int64_t)(k << 1);
+        uint32_t s0, s1, e;
+        if (!sam_field10(p, lines[k].len, s0, s1, e)) return (int64_t)((k << 1) | 1);
+    }
+    return -1;
+}
+
+int sam_threads(size_t n, int asked)
+{
+    int T = asked > 0 ? asked : (int)std::thread::hardware_concurrency();
+    T = std::max(1, std::min(T, 64));
+    return n < (1u << 20) ? 1 : T;
+}
+
+}  // namespace
+
+// pass 1 on the host threads: the same c2b_fastq result as c2b_sam_dedup_gpu_buffer
+extern "C" int c2b_sam_dedup_buffer(const uint8_t *data, size_t n, int32_t n_threads, c2b_fastq **out)
+{
+    if (!out || (n && !data)) return C2B_E_ARG;
+    *out = nullptr;
+    std::vector<TLine> lines;
+    split_text_lines(data, n, lines);
+    const int64_t n_rec = (int64_t)lines.size();
+    if (n_rec >= (int64_t)INT32_MAX / 2) { g_fastq_err = "c2b_sam_dedup_buffer: more than 2^30 lines"; return C2B_E_LIMIT; }
+    const int T = sam_threads(n, n_threads);
+    std::vector<Seq> seq((size_t)n_rec);
+    std::vector<uint64_t> hv((size_t)n_rec);
+    std::vector<int64_t> bad((size_t)T, -1);
+    run_threads(T, [&](int t) {
+        const int64_t lo = n_rec * t / T, hi = n_rec * (t + 1) / T;
+        bad[(size_t)t] = sam_first_bad(data, lines, (size_t)lo, (size_t)hi);
+        if (bad[(size_t)t] >= 0) return;
+        for (int64_t r = lo; r < hi; r++) {
+            const uint8_t *p = data + lines[(size_t)r].p;
+            uint32_t s0, s1, e;
+            sam_field10(p, lines[(size_t)r].len, s0, s1, e);
+            seq[(size_t)r] = Seq{p + s0, s1 - s0};
+            hv[(size_t)r] = hash_bytes(p + s0, s1 - s0);
+        }
+    });
+    for (int64_t b : bad) if (b >= 0) return c2b_sam_line_error(b >> 1, (int)(b & 1));
+    std::unique_ptr<c2b_fastq> F(new c2b_fastq());
+    F->n_reads = n_rec;
+    dedup_records(seq, hv, n_rec, T, F.get(), [](const char *) {});
+    *out = F.release();
+    return C2B_OK;
+}
+
+// pass 2: every line of `text` whose field 10 is a unique read of the handle, as rstrip(line) + "\t" + annotation + "\n", in input
+// order, appended to sam_path (the caller wrote the header); lines whose read is in no table are dropped
+extern "C" int c2b_annotate_write_sam_passthrough(const c2b_annotation *a, const uint8_t *seqs, const int64_t *offsets, int64_t n_unique,
+                                                  const uint8_t *text, size_t n_bytes, const char *sam_path, int32_t n_threads)
+{
+    if (!a || !sam_path || n_unique != a->n || (n_unique && !offsets) || (n_bytes && !text)) {
+        g_fastq_err = "c2b_annotate_write_sam_passthrough: bad argument";
+        return C2B_E_ARG;
+    }
+    std::vector<TLine> lines;
+    split_text_lines(text, n_bytes, lines);
+    const UniqueIndex idx(seqs, offsets, n_unique);
+    const int64_t n_lines = (int64_t)lines.size();
+    const int T = sam_threads(n_bytes, n_threads);
+    std::vector<std::string> outs((size_t)T);
+    std::vector<int64_t> bad((size_t)T, -1);
+    run_threads(T, [&](int t) {
+        const int64_t lo = n_lines * t / T, hi = n_lines * (t + 1) / T;
+        bad[(size_t)t] = sam_first_bad(text, lines, (size_t)lo, (size_t)hi);
+        if (bad[(size_t)t] >= 0) return;
+        std::string &o = outs[(size_t)t];
+        for (int64_t k = lo; k < hi; k++) {
+            const uint8_t *p = text + lines[(size_t)k].p;
+            uint32_t s0, s1, e;
+            sam_field10(p, lines[(size_t)k].len, s0, s1, e);
+            const int64_t u = idx.find(p + s0, s1 - s0);
+            if (u < 0) continue;
+            o.append((const char *)p, e);
+            o.push_back('\t');
+            o.append((const char *)a->ann.data() + a->ann_off[(size_t)u], (size_t)(a->ann_off[(size_t)u + 1] - a->ann_off[(size_t)u]));
+            o.push_back('\n');
+        }
+    });
+    for (int64_t b : bad) if (b >= 0) return c2b_sam_line_error(b >> 1, (int)(b & 1));
+    if (!write_parts(sam_path, outs, std::string(), true)) {
+        g_fastq_err = std::string("c2b_annotate_write_sam_passthrough: cannot write ") + sam_path;
+        return C2B_E_STATE;
     }
     return C2B_OK;
 }

@@ -1,6 +1,9 @@
 // c2b_fastq_gpu.cu -- FASTQ parse + exact de-duplication ON the GPU: the file's bytes cross PCIe once, the unique reads come
 // back packed in first-seen order with their multiplicities (the same c2b_fastq object as the host front end, c2b_fastq.cpp).
 //
+// Also the pass-1 loop of process_bam (c2b_sam_dedup_gpu_buffer): the same passes over SAM text with one record per line and
+// k_sam_records in place of k_records.
+//
 // Replaces: the FASTQ loop of process_fastq (reference: CRISPResso2/CRISPRessoCORE.py:1820-1849), same semantics as
 // c2b_fastq_dedup -- text-mode universal newlines ("\n", "\r\n", a lone "\r"), a record starts at every fourth line that exists
 // and takes the next three lines present or not, the sequence is line 2 stripped of ASCII whitespace, unique sequences in
@@ -9,6 +12,7 @@
 // Passes (one stream; CUB for the scans, the select and the sort):
 //   k_count_ends / k_write_ends   line terminators per 4 KiB tile -> exclusive scan -> position of every line end
 //   k_records                     one thread per record: line 4r+1, stripped -> (start, length, 64-bit hash)
+//   k_sam_records                 (SAM) one warp per line: field 10 of the right-stripped line -> (start, length, hash)
 //   k_dedup                       open-addressing table of record indices (CAS insert, byte-exact compare on a hash match): every
 //                                 record finds its group's representative; atomicMin / atomicAdd give the group's first record
 //                                 and its multiplicity -- exact, no probabilistic step
@@ -115,6 +119,66 @@ __global__ void k_records(const uint8_t *__restrict__ t, int64_t n, const int64_
     for (int64_t p = a; p < b; p++) { h = (h ^ t[p]) * 0x100000001b3ull; }
     h ^= h >> 29; h *= 0xc4ceb9fe1a85ec53ull; h ^= h >> 32;
     rptr[r] = a; rlen[r] = (int32_t)(b - a); rhash[r] = h;
+}
+
+// SAM text (the pass-1 loop of process_bam, CRISPRessoCORE.py:2047-2057): record r = line r, its sequence is
+// line.rstrip().split("\t")[9].  One warp per line, 32-byte windows: ballots of the tabs, of the non-space bytes (the rstrip end
+// is one past the last of them) and of the non-ASCII bytes.  Field 10 starts after the 9th tab and ends at the 10th tab or at
+// the rstrip end, whichever comes first; a 9th tab at or past the rstrip end means fewer than 10 fields (IndexError there).
+// err: atomicMin of (line << 1) | kind over the bad lines, kind 0 = a non-ASCII byte, 1 = fewer than 10 fields.
+// The hash is a sum of per-position terms (any function of the bytes serves: k_dedup decides equality by comparing bytes).
+__global__ void __launch_bounds__(256) k_sam_records(const uint8_t *__restrict__ t, int64_t n, const int64_t *__restrict__ ends,
+                                                     int64_t n_ends, int64_t n_rec, int64_t *__restrict__ rptr,
+                                                     int32_t *__restrict__ rlen, uint64_t *__restrict__ rhash,
+                                                     unsigned long long *__restrict__ err)
+{
+    const int64_t r = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    if (r >= n_rec) return;
+    const int64_t a = r ? ends[r - 1] + 1 : 0;
+    int64_t b = n;
+    if (r < n_ends) { b = ends[r]; if (t[b] == '\n' && b > a && t[b - 1] == '\r') b--; }
+    int tabs = 0;
+    int64_t p9 = -1, p10 = -1, last = a - 1;
+    bool wide = false;
+    for (int64_t w = a; w < b; w += 32) {
+        const int64_t p = w + lane;
+        const uint8_t c = p < b ? __ldg(t + p) : (uint8_t)' ';
+        const uint32_t tb = __ballot_sync(0xffffffffu, c == '\t');
+        const uint32_t ns = __ballot_sync(0xffffffffu, !is_space_d(c));
+        wide |= __ballot_sync(0xffffffffu, c >= 0x80) != 0;
+        if (ns) last = w + 31 - __clz(ns);
+        const int pc = __popc(tb);
+        if (p10 < 0 && tabs + pc >= 9) {                       // the 9th and / or 10th tab fall in this window
+            uint32_t m = tb;
+            for (int k = tabs; k < tabs + pc && k < 10; k++) {
+                const int64_t q = w + __ffs(m) - 1;
+                m &= m - 1;
+                if (k == 8) p9 = q; else if (k == 9) p10 = q;
+            }
+        }
+        tabs += pc;
+    }
+    const int64_t e = last + 1;                                 // rstrip end
+    uint64_t h = 0;
+    int64_t s0 = 0, s1 = 0;
+    const bool shortl = p9 < 0 || p9 >= e;
+    if (!wide && !shortl) {
+        s0 = p9 + 1;
+        s1 = (p10 >= 0 && p10 < e) ? p10 : e;
+        for (int64_t p = s0 + lane; p < s1; p += 32) {
+            uint64_t x = ((uint64_t)__ldg(t + p) << 40) ^ (uint64_t)(p - s0);
+            x *= 0xff51afd7ed558ccdull; x ^= x >> 33; x *= 0xc4ceb9fe1a85ec53ull; x ^= x >> 29;
+            h += x;
+        }
+        for (int d = 16; d; d >>= 1) h += __shfl_xor_sync(0xffffffffu, h, d);
+        h ^= (uint64_t)(s1 - s0) * 0x9E3779B97F4A7C15ull;
+        h ^= h >> 31; h *= 0xff51afd7ed558ccdull; h ^= h >> 32;
+    }
+    if (lane == 0) {
+        if (wide || shortl) atomicMin(err, ((unsigned long long)r << 1) | (wide ? 0ull : 1ull));
+        rptr[r] = s0; rlen[r] = (int32_t)(s1 - s0); rhash[r] = h;
+    }
 }
 
 __global__ void k_dedup(const uint8_t *__restrict__ t, const int64_t *__restrict__ rptr, const int32_t *__restrict__ rlen,
@@ -340,7 +404,8 @@ struct Source {
     }
 };
 
-int dedup_device(const Source &src, size_t n, int device, c2b_fastq **out)
+// sam = false: FASTQ records (k_records); true: one SAM line per record (k_sam_records)
+int dedup_device(const Source &src, size_t n, int device, c2b_fastq **out, bool sam = false)
 {
     const bool verbose = getenv("C2B_FASTQ_VERBOSE") != nullptr;
     auto t_last = std::chrono::steady_clock::now();
@@ -390,7 +455,7 @@ int dedup_device(const Source &src, size_t n, int device, c2b_fastq **out)
     const int64_t n_ends = last_off + last_cnt;
     const bool open_tail = !(last_byte == '\n' || last_byte == '\r');             // the last line has no terminator
     const int64_t n_lines = n_ends + (open_tail ? 1 : 0);
-    const int64_t n_rec = (n_lines + 3) / 4;
+    const int64_t n_rec = sam ? n_lines : (n_lines + 3) / 4;
     if (n_rec >= (int64_t)INT_MAX / 2) { c2b_fastq_set_error("c2b_fastq_dedup_gpu: more than 2^30 records"); return C2B_E_LIMIT; }
     GCHK(d_ends.get((size_t)(n_ends + 1) * 8));
     k_write_ends<<<(unsigned)ntiles, TILE_T, 0, s>>>(d_text.as<uint8_t>(), (int64_t)n, d_to.as<int64_t>(), d_ends.as<int64_t>());
@@ -400,9 +465,22 @@ int dedup_device(const Source &src, size_t n, int device, c2b_fastq **out)
     DBuf d_ptr, d_len, d_hash, d_table, d_first, d_count, d_isrep, d_reps, d_nsel, d_keys, d_keys2, d_reps2, d_lens, d_offs;
     GCHK(d_ptr.get((size_t)n_rec * 8)); GCHK(d_len.get((size_t)n_rec * 4)); GCHK(d_hash.get((size_t)n_rec * 8));
     const unsigned TB = 256, GB = (unsigned)((n_rec + TB - 1) / TB);
-    // line L - 1 of record 0 is line 0: ends[L - 1] is read for L >= 1 only, which k_records guarantees (L = 4r + 1 >= 1)
-    k_records<<<GB, TB, 0, s>>>(d_text.as<uint8_t>(), (int64_t)n, d_ends.as<int64_t>(), n_ends, n_lines, n_rec, d_ptr.as<int64_t>(),
-                                d_len.as<int32_t>(), d_hash.as<uint64_t>());
+    if (!sam) {
+        // line L - 1 of record 0 is line 0: ends[L - 1] is read for L >= 1 only, which k_records guarantees (L = 4r + 1 >= 1)
+        k_records<<<GB, TB, 0, s>>>(d_text.as<uint8_t>(), (int64_t)n, d_ends.as<int64_t>(), n_ends, n_lines, n_rec, d_ptr.as<int64_t>(),
+                                    d_len.as<int32_t>(), d_hash.as<uint64_t>());
+    } else {
+        DBuf d_err;
+        GCHK(d_err.get(8));
+        GCHK(cudaMemsetAsync(d_err.p, 0xff, 8, s));
+        k_sam_records<<<(unsigned)((n_rec * 32 + TB - 1) / TB), TB, 0, s>>>(d_text.as<uint8_t>(), (int64_t)n, d_ends.as<int64_t>(), n_ends,
+                                                                            n_rec, d_ptr.as<int64_t>(), d_len.as<int32_t>(),
+                                                                            d_hash.as<uint64_t>(), d_err.as<unsigned long long>());
+        unsigned long long bad = ~0ull;
+        GCHK(cudaMemcpyAsync(&bad, d_err.p, 8, cudaMemcpyDeviceToHost, s));
+        GCHK(cudaStreamSynchronize(s));
+        if (bad != ~0ull) return c2b_sam_line_error((int64_t)(bad >> 1), (int)(bad & 1));
+    }
     uint32_t cap = 64;
     while ((int64_t)cap < 2 * n_rec + 8) cap <<= 1;
     GCHK(d_table.get((size_t)cap * 4)); GCHK(d_first.get((size_t)n_rec * 4)); GCHK(d_count.get((size_t)n_rec * 4)); GCHK(d_isrep.get((size_t)n_rec));
@@ -472,6 +550,15 @@ extern "C" int c2b_fastq_dedup_gpu_buffer(const uint8_t *data, size_t n, int32_t
     Source src;
     src.mem = data;
     return dedup_device(src, n, device, out);
+}
+
+extern "C" int c2b_sam_dedup_gpu_buffer(const uint8_t *data, size_t n, int32_t device, c2b_fastq **out)
+{
+    if (!out || (n && !data)) return C2B_E_ARG;
+    *out = nullptr;
+    Source src;
+    src.mem = data;
+    return dedup_device(src, n, device, out, true);
 }
 
 extern "C" int c2b_fastq_dedup_gpu(const char *path, int32_t device, c2b_fastq **out)

@@ -43,3 +43,5 @@ struct c2b_annotation {
 // whole file into memory (c2b_fastq.cpp): plain read / gzip inflate (blocked gzip: all host threads)
 bool c2b_fastq_read_gz(const char *path, c2b_bytes &buf, std::string &err);
 void c2b_fastq_set_error(const std::string &m);
+// error of a SAM text line (0-based `line`; kind 0: a non-ASCII byte -> C2B_E_ARG, 1: fewer than 10 fields -> C2B_E_LIMIT)
+int c2b_sam_line_error(int64_t line, int kind);

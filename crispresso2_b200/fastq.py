@@ -75,6 +75,16 @@ def gpu_ingest_device(path, engine_device=None, lib_path=None):
     host threads).  C2B_GPU_INGEST=1 forces the GPU, =0 the host; unset: the GPU when the library has the device front end
     (not the emulator test build) and the file is small enough to sit in HBM whole."""
     import os
+    try:
+        size = os.path.getsize(path)
+    except OSError:
+        size = None
+    return _ingest_rule(size, str(path).endswith(".gz"), engine_device, lib_path)
+
+
+def _ingest_rule(size, gz, engine_device, lib_path):
+    """the rule of gpu_ingest_device for `size` bytes of input (None: unknown size -> the host threads unless forced)"""
+    import os
     dev = 0 if engine_device is None else int(engine_device)
     env = os.environ.get("C2B_GPU_INGEST", "")
     if env == "0":
@@ -83,11 +93,9 @@ def gpu_ingest_device(path, engine_device=None, lib_path=None):
         return dev
     if not _lib.load(lib_path).c2b_fastq_gpu_available():
         return None
-    try:
-        size = os.path.getsize(path)
-    except OSError:
+    if size is None:
         return None
-    return dev if size <= (GPU_INGEST_MAX_GZ if str(path).endswith(".gz") else GPU_INGEST_MAX_PLAIN) else None
+    return dev if size <= (GPU_INGEST_MAX_GZ if gz else GPU_INGEST_MAX_PLAIN) else None
 
 
 def dedup_for_process_fastq(path, engine_device, lib_path=None):
@@ -130,3 +138,36 @@ def dedup_bytes(data, n_threads=0, lib_path=None, device=None):
     if rc != 0:
         raise FastqError("c2b_fastq_dedup%s_buffer failed (%d): %s" % ("_gpu" if device is not None else "", rc, L.c2b_fastq_last_error().decode()))
     return _collect(L, h)
+
+
+def dedup_sam(data, n_threads=0, lib_path=None, device=None):
+    """Pass 1 of process_bam over SAM text (bytes): one record per line, its read is line.rstrip().split("\t")[9]; same result
+    object as dedup_file.  device=None: host threads (c2b_sam_dedup_buffer); device=k: on GPU k (c2b_sam_dedup_gpu_buffer).
+    A line with fewer than 10 fields raises IndexError, as the reference's loop does; a non-ASCII byte raises FastqError."""
+    L = _lib.load(lib_path)
+    h = C.c_void_p()
+    arr = np.frombuffer(data, dtype=np.uint8)
+    ptr = arr.ctypes.data if len(arr) else None
+    if device is not None:
+        rc = L.c2b_sam_dedup_gpu_buffer(ptr, len(arr), int(device), C.byref(h))
+        name = "c2b_sam_dedup_gpu_buffer"
+    else:
+        rc = L.c2b_sam_dedup_buffer(ptr, len(arr), int(n_threads), C.byref(h))
+        name = "c2b_sam_dedup_buffer"
+    if rc == _lib.E_LIMIT:
+        raise IndexError("list index out of range: %s" % L.c2b_fastq_last_error().decode())
+    if rc != 0:
+        raise FastqError("%s failed (%d): %s" % (name, rc, L.c2b_fastq_last_error().decode()))
+    return _collect(L, h)
+
+
+def dedup_for_process_bam(data, engine_device, lib_path=None):
+    """The front end process_bam uses for its pass-1 text: the GPU one by the rule of dedup_for_process_fastq (build and size;
+    C2B_GPU_INGEST=0 / 1 forces either), else the host threads.  A failure of the chosen one raises."""
+    dev = _ingest_rule(len(data), False, engine_device, lib_path)
+    try:
+        return dedup_sam(data, lib_path=lib_path, device=dev)
+    except FastqError as ex:
+        if dev is not None:
+            raise FastqError("%s (GPU SAM front end; C2B_GPU_INGEST=0 selects the host threads)" % ex) from None
+        raise

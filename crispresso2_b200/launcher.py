@@ -9,6 +9,8 @@ What is re-bound (INTEGRATION.md section 2), nothing else of the reference chang
     process_fastq_write_out :2285 and process_single_fastq_write_bam_out :2373)   -> crispresso2_b200.core.process_fastq
   * CRISPRessoCORE.process_fastq_write_out / process_single_fastq_write_bam_out (--fastq_output / --bam_output, :3739-3743)
     -> crispresso2_b200.annotate (single process; under torchrun the reference's wrappers stay bound)
+  * CRISPRessoCORE.process_bam (--bam_input, :3737-3738)   -> crispresso2_b200.bam.process_bam (single process; under torchrun
+    the reference's function stays bound)
   * CRISPRessoCORE.process_paired_fastq (--crispresso_merge, :3744-3748)   -> crispresso2_b200.paired: the reference's loop with its
     global_align calls answered from one GPU batch over every distinct mate sequence
   * filterFastqs.filterFastqs (imported and called at CRISPRessoCORE.py:3716-3717)          -> crispresso2_b200.filter_fastqs.filterFastqs
@@ -86,6 +88,18 @@ def bind(CORE=None, engine=None, lib_path=None):
 
         CORE.process_fastq_write_out = process_fastq_write_out
         CORE.process_single_fastq_write_bam_out = process_single_fastq_write_bam_out
+
+        # --bam_input: the SAM front end, the batch and the annotations on the GPU, the pass-through SAM written natively (bam.py)
+        from . import bam
+
+        def process_bam(bam_filename, bam_chr_loc, output_bam, variantCache, ref_names, refs, args, files_to_remove, output_directory):
+            loc = args.needleman_wunsch_aln_matrix_loc
+            if not os.path.isabs(loc):
+                loc = os.path.join(CORE._ROOT, loc)                 # CRISPRessoCORE.py:2018
+            return bam.process_bam(bam_filename, bam_chr_loc, output_bam, variantCache, ref_names, refs, args, files_to_remove,
+                                   output_directory, engine=get_engine(), aln_matrix=core.read_matrix(loc))
+
+        CORE.process_bam = process_bam
     # paired-end merge mode (--crispresso_merge): the reference's own loop over one batch of GPU alignments (paired.py)
     from . import paired
     reference_paired = CORE.process_paired_fastq

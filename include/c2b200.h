@@ -314,6 +314,14 @@ const char *c2b_fastq_last_error(void);
 int  c2b_fastq_gpu_available(void);              /* 1 in the CUDA build; 0 in the CPU emulator test build (no device front end) */
 int  c2b_fastq_dedup_gpu(const char *path, int32_t device, c2b_fastq **out);
 int  c2b_fastq_dedup_gpu_buffer(const uint8_t *data, size_t n_bytes, int32_t device, c2b_fastq **out);
+/* replaces: the pass-1 loop of process_bam (CRISPRessoCORE.py:2047-2057) over the text of `samtools view -F <flags> <bam>
+ * [<region>]`: one record per line (text-mode universal newlines), its sequence is line.rstrip().split("\t")[9], identical
+ * sequences counted in first-seen order.  Same c2b_fastq result and accessors (n_reads = lines).  A line with fewer than 10
+ * fields returns C2B_E_LIMIT (IndexError in the reference), a non-ASCII byte C2B_E_ARG (out of contract); the first bad line
+ * is named in c2b_fastq_last_error.  _gpu_buffer: line index, one warp per line, exact dedup on the device (C2B_E_STATE in the
+ * emulator build); _buffer: host threads (n_threads <= 0: all). */
+int  c2b_sam_dedup_gpu_buffer(const uint8_t *data, size_t n_bytes, int32_t device, c2b_fastq **out);
+int  c2b_sam_dedup_buffer(const uint8_t *data, size_t n_bytes, int32_t n_threads, c2b_fastq **out);
 
 /* replaces: the reverse-complement count transfer at the head of the quantification loop (CRISPRessoCORE.py:3964-3975) for
  * packed unique reads in first-seen order: weights[k] = the count read k ends up with (0 for a read absorbed by an earlier
@@ -382,7 +390,10 @@ int  c2b_alleles_cut_fetch(const c2b_alleles *a, uint8_t *seq, uint8_t *ref, int
  * amask = slots listed in aln_ref_names (ascending; 0 = not aligned), aname = name id of the one listed slot when it is
  * re-labelled (prime-editing scaffold), else -1, label = class_name id.  names[0..R) are the references' own names;
  * name_rev[id] = refs[name]['aln_strand'] == '-'.  ref_seqs are the R amplicons as aligned.  Uniques go through the device in
- * chunks of `chunk` (<= 0: 65536) through pinned buffers on the engine's stream. */
+ * chunks of `chunk` (<= 0: 65536) through pinned buffers on the engine's stream.  flags: C2B_F_LEGACY_INS, and
+ * C2B_ANN_SAM_OPTIONAL for the form of process_bam (:2217-2234): "c2:Z:" instead of the leading space, no ALN_SCORES /
+ * ALN_DETAILS for aligned reads (not-aligned reads and reads outside the contract keep them). */
+#define C2B_ANN_SAM_OPTIONAL  (1u << 16)
 typedef struct c2b_annotation c2b_annotation;
 int  c2b_annotate_build(c2b_engine *e, const uint8_t *reads, const int64_t *offsets, int64_t n_unique, const int32_t *bidx,
                         int32_t R, int32_t NW, int32_t edit_cap, const c2b_read_rec *recs, const c2b_aln_rec *alns,
@@ -417,6 +428,12 @@ int  c2b_annotate_write_fastq(const c2b_annotation *a, const uint8_t *seqs, cons
 int  c2b_annotate_write_sam(c2b_annotation *a, const uint8_t *seqs, const int64_t *offsets, int64_t n_unique,
                             const char *in_path, const char *sam_path, const char *header, int32_t n_names,
                             const char *const *chr, const char *const *pos, const uint8_t *rev, int32_t n_threads);
+/* replaces: the pass-2 loop of process_bam (:2251-2262) over the text of `samtools view <bam> [<region>]`: every line whose
+ * field 10 is one of the handle's unique reads (seqs / offsets) is appended to sam_path (the caller opened it and wrote the
+ * header) as rstrip(line) + "\t" + annotation + "\n", in input order; other lines are dropped.  The annotations should be built
+ * with C2B_ANN_SAM_OPTIONAL.  Same line rules and errors as c2b_sam_dedup_buffer.  Host threads (n_threads <= 0: all). */
+int  c2b_annotate_write_sam_passthrough(const c2b_annotation *a, const uint8_t *seqs, const int64_t *offsets, int64_t n_unique,
+                                        const uint8_t *text, size_t n_bytes, const char *sam_path, int32_t n_threads);
 
 /* replaces: filterFastqs.filterFastqs for paired input (CRISPResso2/filterFastqs.py:230-407, the seven run_*_pair variants): both
  * files in lockstep, a pair kept iff both mates pass; mate 2 strictly above the threshold when only the min or only the mean

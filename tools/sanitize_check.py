@@ -84,4 +84,11 @@ core.process_fastq(fq, cache, w3.ref_names, w3.refs, a, [], d, engine=eng, aln_m
 A = annotate.Annotation(cache, w3.refs, chunk=700)
 A.write_fastq(fq, os.path.join(d, 'out.fastq.gz'))
 print('annotate', A.n, int(A.ann_off[-1]))
+# --bam_input: the SAM front end (k_sam_records, one warp per line) and the process_bam annotation form, several chunks
+sam = b"".join(b"r%d\t%d\tc\t1\t42\t250M\t*\t0\t0\t%s\tII\tAS:i:0%s" % (k, 16 * (k & 1), s.encode(), [b"\n", b"\r\n", b"\r"][k % 3])
+               for k, s in enumerate(reads[:3000] + reads[:500])) + b"r\t0\tc\t1\t0\t*\t*\t0\t0\tACGT"
+ds, hs = fastq.dedup_sam(sam, device=0), fastq.dedup_sam(sam)
+assert ds.n_reads == hs.n_reads and np.array_equal(ds.buf, hs.buf) and np.array_equal(ds.counts, hs.counts)
+B = annotate.Annotation(cache, w3.refs, chunk=700, sam_optional=True)
+print('sam ingest', ds.n_reads, len(ds.counts), 'annotate sam form', B.n, int(B.ann_off[-1]))
 import shutil; shutil.rmtree(d, ignore_errors=True)
