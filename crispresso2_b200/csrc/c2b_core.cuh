@@ -129,7 +129,17 @@ struct RefDev {
     // edge-run scores of the offsets 1..dg_S on either side is aligned on the main diagonal, no DP needed
     int32_t dg_ok, dg_S, dg_thr4;
     int32_t dg_c4[2 * 4 + 1];      // [s + 4]: 4 x (gap costs + incentives) of the path on offset diagonal s (edge runs only)
+    // routing of the tier's unproved reads (route_read, DESIGN.md section 3): a read whose lower bound on its best one-gap
+    // path does not beat rt_thr (the narrow band's ring_bound at J == I) goes straight to the wide ring
+    int32_t rt_ok, rt_thr;
+    int32_t rt_mx;                 // least match score minus least other score (ACGT codes; everything else never matches)
+    int32_t rt_c[32];              // [s + 16]: gap and edge-run costs of offset s + least score of its I - |s| diagonal columns
+                                   // (RT_OFF: offset not tried -- s == 0, or outside the narrow band)
+    const uint4 *rt_pl;            // [Ipad/32 + 2]: reference codes as bit planes (x: bit 0, y: bit 1, z: code in ACGT), zero past I
 };
+constexpr int32_t RT_OFF = -(1 << 30);
+// the narrow first tier's band (align_narrow16): paths inside column - row in [-RN_DLO, RN_DHI] are computed exactly
+constexpr int RN_DLO = 17, RN_DHI = 11;
 
 struct KParams {
     const uint8_t *reads; const int64_t *offsets; int64_t n_reads;
@@ -154,8 +164,10 @@ struct KParams {
     uint64_t *gops; uint32_t *gmeta; int32_t NW;            // NW = W / 32 words of 32 ops per slot
     int32_t *left; unsigned long long *left_n;              // ALIGN kernel: pairs left over for the general kernel, and their count
     int32_t *left2; unsigned long long *left2_n;            // ALIGN kernel, narrow first tier: reads for the second-tier launch (nullptr: no narrow tier)
-    int32_t *left0; unsigned long long *left0_n;            // diagonal tier: reads it did not prove, for the narrow tier, and their count
-    unsigned long long *diag_n;                             // diagonal tier: [0] reads proved, [1] reads put on its list (cumulative)
+    int32_t *left0; unsigned long long *left0_n;            // diagonal tier: reads it did not prove (CLASSIFY's list), and their count
+    int32_t *left1; unsigned long long *left1_n;            // diagonal tier with routing: the unproved reads it keeps for the narrow tier
+    int32_t route;                                          // diagonal tier: 0 no routing, 1 route_read decides, 2 route every unproved read
+    unsigned long long *diag_n;                             // diagonal tier: [0] reads proved, [1] reads put on its list, [2] tier-2 reads, [3] routed, [4] kept (cumulative)
     const unsigned long long *n_dev;                        // general kernel over the left-over list: *n_dev reads (entries of pair_order)
     int32_t discard_slab;                                   // ALIGN kernel: drop the dead slab lines from L2 instead of writing them back
     unsigned long long *stats;             // cumulative path statistics (c2b_path_counts), indices 2..7; [26] reads sent to the second tier

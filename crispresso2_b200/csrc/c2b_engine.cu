@@ -297,14 +297,20 @@ __global__ void __launch_bounds__(D_WARPS_PER_CTA * 32) c2b_diag_kernel(const __
     ScAcc<1> acc;
     sc_init(acc);
     const int64_t units = (P.n_reads + 31) / 32;
-    int proved = 0, seen = 0;
+    int proved = 0, seen = 0, routed = 0;
     for (int64_t u = (int64_t)blockIdx.x * D_WARPS_PER_CTA + (threadIdx.x >> 5); u < units; u += (int64_t)gridDim.x * D_WARPS_PER_CTA) {
-        proved += diag_unit(P, S, u, acc);
+        int k = 0;
+        proved += diag_unit(P, S, u, acc, k);
+        routed += k;
         seen += P.n_reads - 32 * u < 32 ? (int)(P.n_reads - 32 * u) : 32;
         __syncwarp();
     }
     sc_flush(acc, P);
-    if ((threadIdx.x & 31) == 0 && seen) { wp::addg(P.diag_n, proved); wp::addg(P.diag_n + 1, seen - proved); }
+    if ((threadIdx.x & 31) == 0 && seen) {
+        wp::addg(P.diag_n, proved); wp::addg(P.diag_n + 1, seen - proved);
+        wp::addg(P.diag_n + 2, routed);                  // tier-2 reads: routed here, and the narrow tier's failures
+        wp::addg(P.diag_n + 3, routed); wp::addg(P.diag_n + 4, seen - proved - routed);
+    }
 }
 
 // CLASSIFY kernel (c2b_split.cuh: classify_read): one aligned read per warp, reads strided over the grid -- every read, or
@@ -372,7 +378,7 @@ struct c2b_engine {
     unsigned long long *d_counts = nullptr; size_t counts_n = 0;
     // scratch
     DevBuf tb, tbb, tbq, bnd, ops, rgo, work, lut;
-    DevBuf gops, gmeta, left, left2, left0;   // device-pointer API: op streams / meta words / left-over lists of the last launch
+    DevBuf gops, gmeta, left, left2, left0, left1;   // device-pointer API: op streams / meta words / left-over lists of the last launch
     int n_warps = 0, grid = 0, wpc = 8, stage_cap = 0;
     int grid_a = 0, grid_b = 0, stage_cap_a = 0;       // ALIGN / CLASSIFY kernels
     int split_ok = 0, split_all = 0;                   // configuration admits the two-kernel form (some / all references)
@@ -380,7 +386,7 @@ struct c2b_engine {
     int numa_node = -1;                                // NUMA node of the device (-1: unknown / single node)
     int scratch_TS = 0;
     // staging for the host-pointer API: two buffer sets, copy-in / compute / copy-out streams
-    struct Stage { DevBuf reads, off, cnt, qw, rid, recs, alns, str, ed, maxlen, ord, gops, gmeta, left, left2, left0; int32_t *h_ord = nullptr; size_t h_ord_cap = 0; int64_t *h_off = nullptr; size_t h_off_cap = 0;
+    struct Stage { DevBuf reads, off, cnt, qw, rid, recs, alns, str, ed, maxlen, ord, gops, gmeta, left, left2, left0, left1; int32_t *h_ord = nullptr; size_t h_ord_cap = 0; int64_t *h_off = nullptr; size_t h_off_cap = 0;
                    // pinned bounce buffers for callers whose arrays are pageable (numpy): copies to / from them run on host
                    // threads while the other set's kernels and DMA are in flight
                    uint8_t *h_in = nullptr, *h_out = nullptr; size_t h_in_cap = 0, h_out_cap = 0;
@@ -545,10 +551,10 @@ int c2b_create(int device, c2b_engine **out)
 void c2b_destroy(c2b_engine *e)
 {
     if (!e) return;
-    DevBuf *bufs[] = {&e->tb, &e->tbb, &e->tbq, &e->bnd, &e->ops, &e->rgo, &e->work, &e->lut, &e->gops, &e->gmeta, &e->left, &e->left2, &e->left0};
+    DevBuf *bufs[] = {&e->tb, &e->tbb, &e->tbq, &e->bnd, &e->ops, &e->rgo, &e->work, &e->lut, &e->gops, &e->gmeta, &e->left, &e->left2, &e->left0, &e->left1};
     for (DevBuf *b : bufs) if (b->p) rt_free(b->p);
     for (auto &st : e->stage) {
-        DevBuf *sb[] = {&st.reads, &st.off, &st.cnt, &st.qw, &st.rid, &st.recs, &st.alns, &st.str, &st.ed, &st.maxlen, &st.ord, &st.gops, &st.gmeta, &st.left, &st.left2, &st.left0};
+        DevBuf *sb[] = {&st.reads, &st.off, &st.cnt, &st.qw, &st.rid, &st.recs, &st.alns, &st.str, &st.ed, &st.maxlen, &st.ord, &st.gops, &st.gmeta, &st.left, &st.left2, &st.left0, &st.left1};
         if (st.h_ord) rt_host_free(st.h_ord);
         for (DevBuf *b : sb) if (b->p) rt_free(b->p);
         if (st.h_off) rt_host_free(st.h_off);
@@ -609,6 +615,7 @@ int c2b_configure(c2b_engine *e, const c2b_params *p, int32_t n_refs, const c2b_
         base[r] = bytes;
         bytes += al((size_t)p->nq * Ipad * 4) + 2 * al((size_t)Ipad * 4) + 2 * al(Ipad) + al(Ipad + 1) + 3 * al((size_t)(Ipad + 2) * 2);
         bytes += al((size_t)p->nq * p->nq * Ipad * 4) + 2 * al((size_t)Ipad * 4);      // packed-path tables
+        bytes += al((size_t)(Ipad / 32 + 2) * 16);                                      // routing test's bit planes
     }
     const size_t refs_off = bytes;
     bytes += al(sizeof(RefDev) * n_refs);
@@ -652,6 +659,7 @@ int c2b_configure(c2b_engine *e, const c2b_params *p, int32_t n_refs, const c2b_
         uint32_t *prof2 = (uint32_t *)(hb + o); d.prof2 = (const uint32_t *)(db + o); o += al((size_t)p->nq * p->nq * Ipad * 4);
         uint32_t *cIe2 = (uint32_t *)(hb + o); d.cIe2 = (const uint32_t *)(db + o); o += al((size_t)Ipad * 4);
         uint32_t *g42 = (uint32_t *)(hb + o); d.g42 = (const uint32_t *)(db + o); o += al((size_t)Ipad * 4);
+        uint4 *rt_pl = (uint4 *)(hb + o); d.rt_pl = (const uint4 *)(db + o); o += al((size_t)(Ipad / 32 + 2) * 16);
         const int64_t lim = (1ll << 27);
         for (int q = 0; q < p->nq; q++)
             for (int i = 0; i < I; i++) {
@@ -747,6 +755,45 @@ int c2b_configure(c2b_engine *e, const c2b_params *p, int32_t n_refs, const c2b_
             }
             if (!d.dg_ok) { d.dg_S = 0; d.dg_thr4 = 0; }
         }
+        {   // routing of the diagonal tier's unproved reads (route_read, DESIGN.md section 3)
+            const int nq4 = std::min(p->nq, 4);
+            for (int i = 0; i < I; i++) {                    // bit planes: codes 0..3 match when equal, every other code never
+                const int q = rcode[i];
+                if (q >= nq4) continue;
+                uint4 &w = rt_pl[i >> 5];
+                const uint32_t bit = 1u << (i & 31);
+                if (q & 1) w.x |= bit;
+                if (q & 2) w.y |= bit;
+                w.z |= bit;
+            }
+            // least score of a matched column (reference code < 4, read base equal) and of any other column
+            int64_t m = INT64_MAX, x = INT64_MAX;
+            for (int q = 0; q < p->nq; q++)
+                for (int i = 0; i < I; i++) {
+                    const int64_t v = rf.score_rows[(size_t)q * I + i];
+                    if (q == rcode[i] && q < nq4) m = std::min(m, v); else x = std::min(x, v);
+                }
+            // the narrow tier's bound, ring_bound(P, R, I, RN_DLO, RN_DHI) at J == I
+            const int64_t ge = p->gap_extend, go = p->gap_open, smax = d.rg_smax, gmax = d.rg_gmax, gsum = d.rg_gsum;
+            int64_t thr = -(1 << 28);
+            if (RN_DHI + 1 <= I) thr = std::max(thr, smax * (I - RN_DHI - 1) + (RN_DHI + 1) * (ge + gmax) + (RN_DHI + 1) * ge + gsum);
+            if (RN_DLO + 1 <= I) thr = std::max(thr, smax * (I - RN_DLO - 1) + (RN_DLO + 1) * (ge + gmax) + (RN_DLO + 1) * ge + gsum);
+            const int64_t gI = rf.gap_incentive[I];
+            // every estimate must stay far inside int32: |score| x columns, gap costs, incentives
+            const int64_t big = std::max<int64_t>({std::abs(m == INT64_MAX ? 0 : m), std::abs(x == INT64_MAX ? 0 : x), std::abs(go), std::abs(ge), e->refs[r].gabs});
+            d.rt_ok = d.dg_ok && I <= 256 && m != INT64_MAX && x != INT64_MAX && m > x && big * (4 * I + 64) < (1ll << 28);
+            d.rt_thr = d.rt_ok ? (int32_t)thr : 0;
+            d.rt_mx = d.rt_ok ? (int32_t)(m - x) : 0;
+            for (int k = 0; k < 32; k++) {
+                // offset s = k - 16, t = |s| gap columns; only offsets whose one-gap paths lie inside the narrow band
+                const int s = k - 16, t = s < 0 ? -s : s;
+                const bool on = d.rt_ok && s != 0 && t < I && (s < 0 ? t <= RN_DLO : t <= RN_DHI);
+                // interior gap run (gap_open, then gap_extend) + edge run (s < 0: insertion in row I, gap_extend and
+                // gap_incentive[I] per column; s > 0: deletion in column J, gap_extend per column, gap_incentive[I - t] once)
+                d.rt_c[k] = RT_OFF;
+                if (on) d.rt_c[k] = (int32_t)(go + (t - 1) * ge + (s < 0 ? t * (ge + gI) : t * ge + rf.gap_incentive[I - t]) + x * (I - t));
+            }
+        }
         if (rf.coding_mask)
             for (int q = 0; q < I; q++) incl[q] |= (uint8_t)((rf.coding_mask[q] & 3) << 1);   // after cum[]: bit 0 stays the window
         cumx[0] = cums[0] = 0;
@@ -811,8 +858,9 @@ int c2b_string_width(const c2b_engine *e, int32_t max_read_len)
     return (e->max_I + max_read_len + 31) & ~31;
 }
 
-// work block (u64): [2..7] cumulative path statistics, [24..26] the diagonal tier's (c2b_diag_counts); set s: [8 + 8 s] work
-// hand-out counter, [9 + 8 s] widest alignment, [15 + 8 s] length of the diagonal tier's list
+// work block (u64): [2..7] cumulative path statistics, [24..26] the diagonal tier's (c2b_diag_counts), [27..28] its routing
+// (c2b_route_counts); set s: [8 + 8 s] work hand-out counter, [9 + 8 s] widest alignment, [13 + 8 s] length of the tier-2
+// list, [14 + 8 s] of the narrow tier's list, [15 + 8 s] of the diagonal tier's list
 constexpr size_t WORK_BYTES = 32 * 8;
 
 static int ensure_scratch(c2b_engine *e, int maxJ)
@@ -892,12 +940,13 @@ static int score_range_ok(c2b_engine *e, int64_t maxJ, const char *who)
 // kernel over what ALIGN left over -- or the general kernel alone where the two-kernel form does not apply.  Launches that
 // may overlap in time must use different sets; launches on the same stream are ordered.
 // d_gops / d_gmeta / d_left: op streams [n_reads * R * W/32] u64, meta words [n_reads * R], left-over list [n_reads + 8] i32;
-// d_left2 / d_left0: the narrow tier's and the diagonal tier's lists [n_reads + 16] i32 (nullptr: that tier is off).
+// d_left2 / d_left0 / d_left1: the tier-2 list, the diagonal tier's list and the narrow tier's list after routing, each
+// [n_reads + 16] i32 (nullptr: that tier / routing is off).
 static int launch_on(c2b_engine *e, rt_stream cs, int set, const uint8_t *d_reads, const int64_t *d_offsets, int64_t n_reads,
                      int32_t max_read_len, const int32_t *d_count, const int32_t *d_qweight,
                      const int32_t *d_ref_id, c2b_read_rec *d_recs, c2b_aln_rec *d_alns,
                      uint8_t *d_strings, c2b_edit *d_edits, uint64_t *d_gops, uint32_t *d_gmeta, int32_t *d_left, int32_t *d_left2 = nullptr,
-                     int32_t *d_left0 = nullptr)
+                     int32_t *d_left0 = nullptr, int32_t *d_left1 = nullptr)
 {
     if (!e || !e->configured) return fail(e, C2B_E_STATE, "c2b_align_batch: engine not configured");
     if (n_reads < 0 || !d_recs || !d_alns || (n_reads && (!d_reads || !d_offsets))) return fail(e, C2B_E_ARG, "c2b_align_batch: bad argument");
@@ -974,14 +1023,18 @@ static int launch_on(c2b_engine *e, rt_stream cs, int set, const uint8_t *d_read
         // diagonal tier ahead of the narrow one: reads it proves are done, the narrow tier works through the rest (wk[7] of them).
         // A batch smaller than one narrow unit (16 reads) goes through the groups of eight anyway and keeps them whole.
         const bool diag = narrow && d_left0 && e->diag_any && n_reads >= 16 && !getenv("C2B_NO_DIAG");
+        // routing: the diagonal tier puts the reads the narrow band cannot prove straight on the tier-2 list (wk[5]) and the
+        // rest on the narrow tier's list (wk[6]); CLASSIFY still takes all its unproved reads (wk[7])
+        const bool route = diag && d_left1 && !getenv("C2B_NO_ROUTE");
         if (diag) {
             KParams D = P;
             D.left0 = d_left0; D.left0_n = wk + 7; D.diag_n = P.stats + 24;
+            if (route) { D.left1 = d_left1; D.left1_n = wk + 6; D.left2 = d_left2; D.left2_n = wk + 5; D.route = getenv("C2B_ROUTE_ALL") ? 2 : 1; }
             const int64_t units = (n_reads + 31) / 32;
             const int grid_d = (int)std::min<int64_t>((units + D_WARPS_PER_CTA - 1) / D_WARPS_PER_CTA, (int64_t)e->grid_a * 16);
             c2b_diag_kernel<<<grid_d, D_WARPS_PER_CTA * 32, 0, cs>>>(D);
             e->launches++;
-            A.pair_order = d_left0; A.n_dev = wk + 7;
+            A.pair_order = route ? d_left1 : d_left0; A.n_dev = route ? wk + 6 : wk + 7;
         }
         c2b_align_kernel<<<e->grid_a, e->wpc * 32, smem_a, cs>>>(A);
         KParams B = P;                                        // CLASSIFY: every read in batch order, or the diagonal tier's list
@@ -1017,29 +1070,37 @@ static int launch_on(c2b_engine *e, rt_stream cs, int set, const uint8_t *d_read
             emu::run_warp([&]() { asmem_init(A, AS); });
             const bool narrow = d_left2 && !P.pair_order && (e->n_refs == 1 || d_ref_id != nullptr) && !getenv("C2B_NO_NARROW");
             const int32_t *order = nullptr;                   // CLASSIFY's read order (nullptr: all reads)
-            int64_t n1 = n_reads;
+            int64_t n1 = n_reads;                             // reads CLASSIFY takes
             if (narrow) {
                 A.left2 = d_left2; A.left2_n = wk + 5;
+                int64_t na = n_reads;                         // reads the narrow tier takes
                 if (d_left0 && e->diag_any && n_reads >= 16 && !getenv("C2B_NO_DIAG")) {    // diagonal tier, then the narrow tier over its list
+                    const bool route = d_left1 && !getenv("C2B_NO_ROUTE");
                     KParams D = P;
                     D.left0 = d_left0; D.left0_n = wk + 7; D.diag_n = P.stats + 24;
+                    if (route) { D.left1 = d_left1; D.left1_n = wk + 6; D.left2 = d_left2; D.left2_n = wk + 5; D.route = getenv("C2B_ROUTE_ALL") ? 2 : 1; }
                     static DSmem DS;
                     for (int64_t u = 0; 32 * u < n_reads; u++)
                         emu::run_warp([&]() {
                             dsmem_init(D, DS);
                             ScAcc<1> acc; sc_init(acc);
-                            const int k = diag_unit(D, DS, u, acc), m = n_reads - 32 * u < 32 ? (int)(n_reads - 32 * u) : 32;
+                            int kr = 0;
+                            const int k = diag_unit(D, DS, u, acc, kr), m = n_reads - 32 * u < 32 ? (int)(n_reads - 32 * u) : 32;
                             sc_flush(acc, D);
-                            if (wp::lane() == 0) { wp::addg(D.diag_n, k); wp::addg(D.diag_n + 1, m - k); }
+                            if (wp::lane() == 0) {
+                                wp::addg(D.diag_n, k); wp::addg(D.diag_n + 1, m - k);
+                                wp::addg(D.diag_n + 2, kr); wp::addg(D.diag_n + 3, kr); wp::addg(D.diag_n + 4, m - k - kr);
+                            }
                         });
-                    A.pair_order = d_left0; A.n_dev = wk + 7; n1 = (int64_t)wk[7]; order = d_left0;
+                    A.pair_order = route ? d_left1 : d_left0; A.n_dev = route ? wk + 6 : wk + 7;
+                    na = (int64_t)*A.n_dev; n1 = (int64_t)wk[7]; order = d_left0;
                 }
-                for (int64_t w = 0; 16 * w < n1; w++)
+                for (int64_t w = 0; 16 * w < na; w++)
                     emu::run_warp([&]() {
                         if (!align_narrow16(A, AS, nullptr, w, 0)) {
                             align_group(A, AS, nullptr, 2 * w, 0);
                             wp::sync();
-                            if (8 * (2 * w + 1) < n1) align_group(A, AS, nullptr, 2 * w + 1, 0);
+                            if (8 * (2 * w + 1) < na) align_group(A, AS, nullptr, 2 * w + 1, 0);
                         }
                     });
                 KParams A2 = A;
@@ -1083,7 +1144,8 @@ static int launch_on(c2b_engine *e, rt_stream cs, int set, const uint8_t *d_read
 }
 
 // op-stream buffers of the device-pointer API (engine-owned, sized for the batch)
-static int ensure_ops(c2b_engine *e, DevBuf &gops, DevBuf &gmeta, DevBuf &left, DevBuf &left2, DevBuf &left0, int64_t n_reads, int nr, int W)
+static int ensure_ops(c2b_engine *e, DevBuf &gops, DevBuf &gmeta, DevBuf &left, DevBuf &left2, DevBuf &left0, DevBuf &left1, int64_t n_reads,
+                      int nr, int W)
 {
     int rc;
     if ((rc = ensure(e, gops, (size_t)n_reads * nr * (W / 32) * 8))) return rc;
@@ -1091,6 +1153,7 @@ static int ensure_ops(c2b_engine *e, DevBuf &gops, DevBuf &gmeta, DevBuf &left, 
     if ((rc = ensure(e, left, (size_t)(n_reads + 8) * 4))) return rc;
     if ((rc = ensure(e, left2, (size_t)(n_reads + 16) * 4))) return rc;
     if ((rc = ensure(e, left0, (size_t)(n_reads + 16) * 4))) return rc;
+    if ((rc = ensure(e, left1, (size_t)(n_reads + 16) * 4))) return rc;
     return C2B_OK;
 }
 
@@ -1105,11 +1168,11 @@ int c2b_align_batch_device(c2b_engine *e, const uint8_t *d_reads, const int64_t 
 #endif
     if (max_read_len < 1) max_read_len = 1;
     const int W = (e->max_I + max_read_len + 31) & ~31, nr = d_ref_id ? 1 : e->n_refs;
-    int rc = ensure_ops(e, e->gops, e->gmeta, e->left, e->left2, e->left0, n_reads, nr, W);
+    int rc = ensure_ops(e, e->gops, e->gmeta, e->left, e->left2, e->left0, e->left1, n_reads, nr, W);
     if (rc) return rc;
     return launch_on(e, e->stream, 0, d_reads, d_offsets, n_reads, max_read_len, d_count, d_qweight, d_ref_id, d_recs,
                      d_alns, d_strings, d_edits, (uint64_t *)e->gops.p, (uint32_t *)e->gmeta.p, (int32_t *)e->left.p, (int32_t *)e->left2.p,
-                     (int32_t *)e->left0.p);
+                     (int32_t *)e->left0.p, (int32_t *)e->left1.p);
 }
 
 int c2b_ops_device(c2b_engine *e, void **d_ops, void **d_meta)
@@ -1179,6 +1242,17 @@ int c2b_diag_counts(c2b_engine *e, int64_t *proved, int64_t *tier1, int64_t *tie
     if (proved) *proved = v[0];
     if (tier1) *tier1 = v[1];
     if (tier2) *tier2 = v[2];
+    return C2B_OK;
+}
+
+int c2b_route_counts(c2b_engine *e, int64_t *routed, int64_t *kept)
+{
+    if (!e || !e->work.p) return fail(e, C2B_E_STATE, "c2b_route_counts: nothing launched yet");
+    int64_t v[2] = {0, 0};
+    RTCHK(rt_d2h(v, (unsigned long long *)e->work.p + 27, sizeof v, e->stream));
+    RTCHK(rt_sync(e->stream));
+    if (routed) *routed = v[0];
+    if (kept) *kept = v[1];
     return C2B_OK;
 }
 
@@ -1363,7 +1437,7 @@ static int align_batch_host(c2b_engine *e, const uint8_t *reads, const int64_t *
         if (count && (rc = ensure(e, st.cnt, (size_t)n * 4))) return rc;
         if (qweight && (rc = ensure(e, st.qw, (size_t)n * 4))) return rc;
         if (ref_id && (rc = ensure(e, st.rid, (size_t)n * 4))) return rc;
-        if ((rc = ensure_ops(e, st.gops, st.gmeta, st.left, st.left2, st.left0, n, nr, W))) return rc;
+        if ((rc = ensure_ops(e, st.gops, st.gmeta, st.left, st.left2, st.left0, st.left1, n, nr, W))) return rc;
         if (st.h_off_cap < (size_t)(n + 1)) {
             if (st.h_off) rt_host_free(st.h_off);
             st.h_off = (int64_t *)rt_host_alloc((size_t)(n + 1) * 8); st.h_off_cap = st.h_off ? (size_t)(n + 1) : 0;
@@ -1421,7 +1495,8 @@ static int align_batch_host(c2b_engine *e, const uint8_t *reads, const int64_t *
                        count ? (const int32_t *)st.cnt.p : nullptr, qweight ? (const int32_t *)st.qw.p : nullptr,
                        ref_id ? (const int32_t *)st.rid.p : nullptr, (c2b_read_rec *)st.recs.p,
                        (c2b_aln_rec *)st.alns.p, strings ? (uint8_t *)st.str.p : nullptr,
-                       cap ? (c2b_edit *)st.ed.p : nullptr, (uint64_t *)st.gops.p, (uint32_t *)st.gmeta.p, (int32_t *)st.left.p, (int32_t *)st.left2.p, (int32_t *)st.left0.p);
+                       cap ? (c2b_edit *)st.ed.p : nullptr, (uint64_t *)st.gops.p, (uint32_t *)st.gmeta.p, (int32_t *)st.left.p, (int32_t *)st.left2.p, (int32_t *)st.left0.p,
+                       (int32_t *)st.left1.p);
         e->pair_order = nullptr;
         if (rc) return rc;
         // keep this batch's "widest alignment" before the next launch sequence resets it

@@ -463,6 +463,7 @@ C2B_DEV void align_group(const KParams &P, ASmem &S, const uint32_t *staged_prof
 C2B_DEV bool align_narrow16(const KParams &P, ASmem &S, const uint32_t *staged_prof, int64_t w16, int warp_slot)
 {
     constexpr int RL = 4, DLO = 4 * RL + 1, DHI = 9 * RL - 4 * RL - 9;
+    static_assert(DLO == RN_DLO && DHI == RN_DHI, "the diagonal tier's routing test assumes this band");
     const int lane = wp::lane(), g = lane >> 2;
     const int64_t first = 16 * w16;                         // first read
     if (!P.left2 || P.tbq == nullptr || first + 15 >= nreads(P) || (P.ref_id == nullptr && P.n_refs > 1)) return false;
@@ -1113,8 +1114,12 @@ C2B_DEV void classify_read(const KParams &P, int64_t rd, const BPre &pre, const 
 // its two edge runs.  Then the diagonal is the unique optimum and the reference's traceback returns it (DESIGN.md section 3).
 // The tier also classifies the reads it proves (diag_classify), so the narrow tier and CLASSIFY only see the others.
 // One read per warp, 32 consecutive reads per unit; the unit's unproved reads go, in order and with one atomic, on the tier-0
-// list (P.left0) that the narrow tier and CLASSIFY work through.
+// list (P.left0) that CLASSIFY works through.  With routing (P.route) each of them also goes either on the narrow tier's list
+// (P.left1) or straight onto the tier-2 list (P.left2) that the wide ring works through (route_read).
+constexpr int DG_PROVED = 0, DG_KEEP = 1, DG_ROUTE = 2;     // diag_read: proved / for the narrow tier / for the wide ring
 struct DSmem {                                         // diagonal tier, per warp
+    uint4 pl[2][10];                                   // route_read: the read's and the reference's codes as bit planes, 32 columns per word
+    int32_t pl_ref;                                    // reference whose planes are in pl[1] (-1: none)
     uint8_t fw[RG_COMBO], rc[RG_COMBO];
     uint8_t lut[256];
     int64_t off[33];
@@ -1204,19 +1209,101 @@ C2B_DEV void diag_classify(const KParams &P, const DSmem &S, const RefDev &R, co
     if (lane == 0) P.recs[rd] = rec;
 }
 
-// true if read rd is proved (op stream, meta word and classification written); all lanes call with warp-uniform arguments
-C2B_DEV bool diag_read(const KParams &P, DSmem &S, int64_t rd, int64_t off, int J, int r, long long cnt, long long w, ScAcc<1> &A)
+// Routing test for an unproved read of the amplicon's length (J == I <= 256, every base in the alphabet, one strand); D: its
+// exact score on the main diagonal.  -> DG_KEEP when a path inside the narrow band provably beats that tier's bound (so the
+// narrow tier settles the read), DG_ROUTE otherwise.  The paths tried: the main diagonal up to split p >= 1, one interior gap
+// run of t = |s| columns, offset diagonal s (read j = reference i + s) to the end, then s's edge run.  Index x counts read
+// columns for s < 0 (read x against reference x + t) and reference rows for s > 0 (reference x against read x + t); with m0 /
+// ms the match bits of diagonal 0 / s over x, F(p) = (m0 below p) + (ms from p on), and the path scores at least
+// rt_mx F(p) + rt_c[s] + its gap run's incentives (a matched column scores at least the least match score, any other column
+// at least the least score).  Lane s + 16 takes offset s and finds its best split among the block ends p = 32, 64, ..
+// (clamped to I - t); the best lane's 64 splits around its block end are then scanned exactly, incentives included.  A read
+// is kept iff that lower bound beats rt_thr; any other read costs the wide ring what the narrow tier would have wasted on it.
+C2B_DEV int route_read(const KParams &P, DSmem &S, const RefDev &R, int r, const uint8_t *c, int D)
+{
+    if (!R.rt_ok || D > R.rt_thr) return DG_KEEP;            // no bound for this reference / the diagonal alone beats it
+    const int lane = wp::lane(), I = R.I, nb = (I + 31) >> 5;
+    auto match = [](uint4 a, uint4 b) { return ~((a.x ^ b.x) | (a.y ^ b.y)) & a.z & b.z; };
+    auto shifted = [](uint4 lo, uint4 hi, int t) {           // columns x + t of the word pair (lo, hi), 0 <= t < 32
+        return make_uint4(wp::funnel_r(lo.x, hi.x, t), wp::funnel_r(lo.y, hi.y, t), wp::funnel_r(lo.z, hi.z, t), 0u);
+    };
+    auto below = [](int n) -> uint32_t { return n >= 32 ? ~0u : n <= 0 ? 0u : (1u << n) - 1u; };
+    // bit planes of the read (aligned strand) and, once per reference, of the amplicon; words nb and nb + 1 are zero
+    for (int b = 0; b < nb; b++) {
+        const int x = 32 * b + lane, q = x < I ? c[x] : 255;
+        const uint32_t p0 = wp::ballot(q & 1), p1 = wp::ballot(q & 2), v = wp::ballot(q < 4);
+        if (lane == 0) S.pl[0][b] = make_uint4(p0, p1, v, 0u);
+    }
+    if (lane < 2) S.pl[0][nb + lane] = make_uint4(0u, 0u, 0u, 0u);
+    const bool fresh = S.pl_ref != r;
+    wp::sync();
+    if (fresh) {
+        if (lane < nb + 2) S.pl[1][lane] = R.rt_pl[lane];
+        if (lane == 0) S.pl_ref = r;
+    }
+    wp::sync();
+    const int s = lane - 16, t = s < 0 ? -s : s, cs = R.rt_c[lane];
+    const uint4 *Ap = S.pl[s < 0 ? 0 : 1], *Bp = S.pl[s < 0 ? 1 : 0];
+    int run = 0, best = RT_OFF, bb = 1, mst = 0;             // run: F(32 (b + 1)) - mst; bb: first block end attaining best
+#pragma unroll 1
+    for (int b = 0; b < nb; b++) {
+        const uint32_t m0 = match(S.pl[0][b], S.pl[1][b]) & below(I - t - 32 * b);
+        const uint32_t ms = match(Ap[b], shifted(Bp[b], Bp[b + 1], t));
+        const int k = wp::popc(ms);
+        run += wp::popc(m0) - k; mst += k;
+        if (run > best) { best = run; bb = b + 1; }
+    }
+    const int val = cs == RT_OFF ? RT_OFF : R.rt_mx * (mst + best) + cs;
+    int vmax = val;
+#pragma unroll
+    for (int d = 16; d >= 1; d >>= 1) { const int o = wp::shfl_xor(vmax, d); if (o > vmax) vmax = o; }
+    if (vmax == RT_OFF) return DG_ROUTE;                     // no offset to try: the diagonal alone, which does not beat the bound
+    const int L = wp::ffs(wp::ballot(val == vmax)) - 1;
+    const int s1 = L - 16, t1 = s1 < 0 ? -s1 : s1, w0 = wp::shfl(bb, L) - 1, F1 = wp::shfl(mst + best, L), c1 = wp::shfl(cs, L);
+    const uint4 *A1 = S.pl[s1 < 0 ? 0 : 1], *B1 = S.pl[s1 < 0 ? 1 : 0];
+    uint32_t m0w[2], msw[2];
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+        m0w[h] = match(S.pl[0][w0 + h], S.pl[1][w0 + h]) & below(I - t1 - 32 * (w0 + h));
+        msw[h] = match(A1[w0 + h], shifted(B1[w0 + h], B1[w0 + h + 1], t1));
+    }
+    // lane l: columns 2l, 2l + 1 of blocks w0, w0 + 1; F at the splits after them from F(32 w0) and a prefix sum over the lanes
+    const int F0 = F1 - (wp::popc(m0w[0]) - wp::popc(msw[0]));
+    const uint32_t a = lane < 16 ? m0w[0] : m0w[1], bm = lane < 16 ? msw[0] : msw[1];
+    const int j = (2 * lane) & 31;
+    const int e0 = (int)((a >> j) & 1u) - (int)((bm >> j) & 1u), e1 = (int)((a >> (j + 1)) & 1u) - (int)((bm >> (j + 1)) & 1u);
+    int incl = e0 + e1;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) { const int v = wp::shfl_up(incl, d); if (lane >= d) incl += v; }
+    const int imul = s1 < 0 ? 1 : t1;                        // a deletion collects its row's incentive once, an insertion per column
+    int e = RT_OFF;
+    auto cand = [&](int p, int F) {
+        if (p >= 1 && p <= I - t1) { const int v = R.rt_mx * F + imul * (R.g4[p] >> 2) + c1; if (v > e) e = v; }
+    };
+    const int pa = 32 * w0 + 2 * lane + 1;
+    cand(pa, F0 + incl - e1);
+    cand(pa + 1, F0 + incl);
+    if (lane == 0) cand(32 * w0, F0);
+#pragma unroll
+    for (int d = 16; d >= 1; d >>= 1) { const int o = wp::shfl_xor(e, d); if (o > e) e = o; }
+    return e > R.rt_thr ? DG_KEEP : DG_ROUTE;
+}
+
+// DG_PROVED if read rd is proved (op stream, meta word and classification written), else where it goes next (DG_KEEP: the
+// narrow tier, DG_ROUTE: straight to the wide ring; DG_KEEP whenever routing is off); all lanes call with warp-uniform arguments
+C2B_DEV int diag_read(const KParams &P, DSmem &S, int64_t rd, int64_t off, int J, int r, long long cnt, long long w, ScAcc<1> &A)
 {
     const int lane = wp::lane();
     const RefDev &R = refdev(P, r);
     const int I = R.I;
     // the reads the narrow tier would take (one candidate reference, packed ring admissible), of the amplicon's length
-    if (!R.dg_ok || J != I || J > RG_COMBO || J + 32 > P.TS || J > R.pk_maxJ || I + J > PK_MAX_ALN) return false;
+    if (!R.dg_ok || J != I || J > RG_COMBO || J + 32 > P.TS || J > R.pk_maxJ || I + J > PK_MAX_ALN) return DG_KEEP;
     const bool bad = load_codes_a(P, S.lut, off, J, S.fw, S.rc);
     wp::sync();
-    if (bad) return false;
+    // a symbol outside the alphabet or a seed test that wants both strands: the narrow tier only carries such a read to tier 2
+    if (bad) return P.route ? DG_ROUTE : DG_KEEP;
     const int mode = strand_mode(P, R, S.fw, J);
-    if (mode == 2) return false;                     // both strands: the DP decides which one
+    if (mode == 2) return P.route ? DG_ROUTE : DG_KEEP;     // both strands: the DP decides which one
     const uint8_t *c = mode == 1 ? S.rc : S.fw;
     const int32_t *prof = R.prof;                    // [q][Ipad]: 4 x matrix[reference row][alphabet[q]]
     const int Ipad = R.Ipad, dS = R.dg_S;
@@ -1239,7 +1326,7 @@ C2B_DEV bool diag_read(const KParams &P, DSmem &S, int64_t rd, int64_t off, int 
 #pragma unroll
     for (int s = -4; s <= 4; s++)
         if (s != 0 && (s < 0 ? -s : s) <= dS) proved = proved && acc[4] > acc[s + 4] + R.dg_c4[s + 4];
-    if (!proved) return false;
+    if (!proved) return P.route == 0 ? DG_KEEP : P.route == 2 ? DG_ROUTE : route_read(P, S, R, r, c, acc[4] >> 2);
     // what align_narrow16 writes for an all-M traceback of I columns: op words of 32 ops, OP_NONE (3) past the end
     const int64_t slot = oslot(P, rd, r);
     if (lane < 16 && lane < P.NW) {
@@ -1248,17 +1335,30 @@ C2B_DEV bool diag_read(const KParams &P, DSmem &S, int64_t rd, int64_t off, int 
     }
     if (lane == 0) P.gmeta[slot] = gmeta_pack(I, mode == 1, GM_ALIGNED);
     diag_classify(P, S, R, c, rd, r, mode == 1, cnt, w, A);
-    return true;
+    return DG_PROVED;
 }
 
 C2B_DEV void dsmem_init(const KParams &P, DSmem &S)
 {
     for (int k = wp::lane(); k < 256; k += 32) S.lut[k] = P.lut[k];
+    if (wp::lane() == 0) S.pl_ref = -1;
     wp::sync();
 }
 
-// reads 32u .. 32u+31: returns the number proved; A: the warp's scalar accumulators (flushed by the caller)
-C2B_DEV int diag_unit(const KParams &P, DSmem &S, int64_t u, ScAcc<1> &A)
+// warp-aggregated append of reads first + x (bit x of mask) to a list: one atomic, the reads stay in order
+C2B_DEV void list_append(int32_t *list, unsigned long long *n, uint32_t mask, int64_t first)
+{
+    if (!mask) return;
+    const int lane = wp::lane();
+    unsigned long long pos = 0;
+    if (lane == 0) pos = wp::fetch_add(n, (unsigned long long)wp::popc(mask));
+    pos = (unsigned long long)(uint32_t)wp::shfl((int)(uint32_t)pos, 0) | ((unsigned long long)(uint32_t)wp::shfl((int)(uint32_t)(pos >> 32), 0) << 32);
+    if ((mask >> lane) & 1u) list[pos + wp::popc(mask & ((1u << lane) - 1u))] = (int32_t)(first + lane);
+}
+
+// reads 32u .. 32u+31: returns the number proved, `routed` the number sent straight to tier 2; A: the warp's scalar
+// accumulators (flushed by the caller)
+C2B_DEV int diag_unit(const KParams &P, DSmem &S, int64_t u, ScAcc<1> &A, int &routed)
 {
     const int lane = wp::lane();
     const int64_t first = 32 * u;
@@ -1278,19 +1378,21 @@ C2B_DEV int diag_unit(const KParams &P, DSmem &S, int64_t u, ScAcc<1> &A)
         for (int64_t a = b0 + (int64_t)lane * 128; a < b1; a += 32 * 128) asm volatile("prefetch.global.L2 [%0];" ::"l"(P.reads + a));
     }
 #endif
-    uint32_t fail = 0;
+    uint32_t fail = 0, route = 0;
 #pragma unroll 1
     for (int x = 0; x < n; x++) {
         const int64_t off = S.off[x];
-        if (!diag_read(P, S, first + x, off, (int)(S.off[x + 1] - off), S.ref[x], S.cnt[x], S.qw[x], A)) fail |= 1u << x;
+        const int v = diag_read(P, S, first + x, off, (int)(S.off[x + 1] - off), S.ref[x], S.cnt[x], S.qw[x], A);
+        if (v != DG_PROVED) fail |= 1u << x;
+        if (v == DG_ROUTE) route |= 1u << x;
         wp::sync();
     }
-    if (fail) {                                      // warp-aggregated append: the unit's leftovers stay in read order
-        unsigned long long pos = 0;
-        if (lane == 0) pos = wp::fetch_add(P.left0_n, (unsigned long long)wp::popc(fail));
-        pos = (unsigned long long)(uint32_t)wp::shfl((int)(uint32_t)pos, 0) | ((unsigned long long)(uint32_t)wp::shfl((int)(uint32_t)(pos >> 32), 0) << 32);
-        if ((fail >> lane) & 1u) P.left0[pos + wp::popc(fail & ((1u << lane) - 1u))] = (int32_t)(first + lane);
+    list_append(P.left0, P.left0_n, fail, first);   // every unproved read: CLASSIFY's list
+    if (P.route) {                                   // routing: the narrow tier's list and the tier-2 list
+        list_append(P.left1, P.left1_n, fail & ~route, first);
+        list_append(P.left2, P.left2_n, route, first);
     }
+    routed = wp::popc(route);
     return n - wp::popc(fail);
 }
 

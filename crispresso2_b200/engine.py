@@ -287,11 +287,18 @@ class Engine:
         return a.value, b.value
 
     def diag_counts(self):
-        """(reads proved on the main diagonal, reads the diagonal tier handed to the narrow tier, reads the narrow tier sent
-        to the wide ring) since the last counts_reset"""
+        """(reads proved on the main diagonal, reads the diagonal tier did not prove, reads that went on to the wide ring --
+        routed there by the diagonal tier or sent by the narrow tier) since the last counts_reset"""
         a, b, c = C.c_int64(0), C.c_int64(0), C.c_int64(0)
         self._check(self.L.c2b_diag_counts(self.h, C.byref(a), C.byref(b), C.byref(c)), "c2b_diag_counts")
         return a.value, b.value, c.value
+
+    def route_counts(self):
+        """(reads the diagonal tier sent straight to the wide ring, unproved reads it kept for the narrow tier) since the
+        last counts_reset"""
+        a, b = C.c_int64(0), C.c_int64(0)
+        self._check(self.L.c2b_route_counts(self.h, C.byref(a), C.byref(b)), "c2b_route_counts")
+        return a.value, b.value
 
     def launch_count(self):
         return int(self.L.c2b_launch_count(self.h))

@@ -257,10 +257,13 @@ int64_t c2b_band_reruns(c2b_engine *e);
 /* pairs aligned by the ring-banded DP (four pairs per warp, band proven sufficient by a score bound) / pairs of
  * ring-eligible groups that fell back to the full matrix (as of the last c2b_path_counts) */
 int  c2b_ring_counts(c2b_engine *e, int64_t *ring_pairs, int64_t *ring_fallbacks);
-/* reads since the last c2b_counts_reset that the diagonal tier proved aligned on the main diagonal / that it handed to the
- * narrow first tier (0 while the tier does not run: C2B_NO_DIAG, no eligible reference) / that the narrow first tier sent
- * on to the wide-ring second tier */
+/* reads since the last c2b_counts_reset that the diagonal tier proved aligned on the main diagonal / that it did not prove
+ * (0 while the tier does not run: C2B_NO_DIAG, no eligible reference) / that went on to the wide-ring second tier, routed
+ * there by the diagonal tier or sent by the narrow first tier */
 int  c2b_diag_counts(c2b_engine *e, int64_t *proved, int64_t *tier1, int64_t *tier2);
+/* of the reads the diagonal tier did not prove since the last c2b_counts_reset: those it sent straight to the wide-ring
+ * second tier (its routing test: C2B_NO_ROUTE switches it off) / those it kept for the narrow first tier */
+int  c2b_route_counts(c2b_engine *e, int64_t *routed, int64_t *kept);
 
 /* replaces: the count vectors / counters built by the quantification loop (CRISPRessoCORE.py:3841-3907,
  * :3964-4115).  Layout above.  c2b_counts_device exposes the block for an NCCL all-reduce.            */

@@ -4,10 +4,12 @@ Runs the workload under torch.profiler (CUDA activity only, nothing else timed i
 time per launch of every kernel by name, the launch order of one step, the diagonal tier's read counts per step and
 the card with its power limit: means over the profiled steps.
 
-  python tools/kernel_times.py [--reads 1048576] [--steps 20] [--warmup 3] [--mix bench|proved|unproved] [--json OUT]
+  python tools/kernel_times.py [--reads 1048576] [--steps 20] [--warmup 3] [--mix bench|proved|unproved] [--route-report] [--json OUT]
 
 --mix replaces the bench's reads (same amplicon, same count): `proved` = reads as long as the amplicon with 0-2
 substitutions and no gap (what the diagonal tier proves), `unproved` = the bench's deletion and insertion templates only.
+--route-report repeats the steps with C2B_NO_ROUTE=1 and prints both kernel tables and the routing test's false-narrow reads
+(kept for the narrow tier, failed there) and false-wide reads (sent to the wide ring, would have passed the narrow tier).
 """
 import argparse
 import json
@@ -58,6 +60,8 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--mix", default="bench", choices=["bench", "proved", "unproved"])
     ap.add_argument("--json", help="also write the table as JSON here")
+    ap.add_argument("--route-report", action="store_true",
+                    help="also run the steps with C2B_NO_ROUTE=1 and report the diagonal tier's false-narrow / false-wide routing")
     args = ap.parse_args()
 
     import numpy as np
@@ -92,65 +96,102 @@ def main():
         if rc != 0:
             raise RuntimeError(L.c2b_last_error(eng.h).decode())
 
-    for _ in range(args.warmup):
-        eng.counts_reset()
-        step()
-    eng.sync()
-    torch.cuda.synchronize(dev)
-    eng.counts_reset()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        for _ in range(args.steps):
+    def measure():
+        """-> (per-launch rows, sum, diag counts per step, route counts per step) of args.steps profiled steps"""
+        for _ in range(args.warmup):
+            eng.counts_reset()
             step()
         eng.sync()
         torch.cuda.synchronize(dev)
+        eng.counts_reset()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for _ in range(args.steps):
+                step()
+            eng.sync()
+            torch.cuda.synchronize(dev)
 
-    # kernels in launch order; every step launches the same sequence, so position k of a step names one launch (the ALIGN
-    # kernel runs twice per step: narrow tier, then wide ring)
-    evs = [ev for ev in prof.events() if ev.device_type.name == "CUDA" and "c2b_" in ev.name]
-    evs.sort(key=lambda ev: ev.time_range.start)
-    if not evs or len(evs) % args.steps:
-        raise SystemExit("kernel_times: %d kernel records for %d steps" % (len(evs), args.steps))
-    per_step = len(evs) // args.steps
-    per = defaultdict(list)
-    names = []
-    for k, ev in enumerate(evs):
-        short = ev.name.split("(")[0].replace("void ", "")
-        key = (k % per_step, short)
-        if k < per_step:
-            names.append(key)
-        per[key].append(ev.time_range.elapsed_us() / 1000.0)
-    rows = []
-    total = 0.0
-    for key in names:
-        v = per[key]
-        if len(v) != args.steps:
-            raise SystemExit("kernel_times: launch sequence differs between steps")
-        ms = sum(v) / len(v)
-        total += ms
-        rows.append({"launch": key[0] + 1, "kernel": key[1], "ms_per_launch": ms})
-
-    diag = None
-    if hasattr(L, "c2b_diag_counts"):
+        # kernels in launch order; every step launches the same sequence, so position k of a step names one launch (the ALIGN
+        # kernel runs twice per step: narrow tier, then wide ring)
+        evs = [ev for ev in prof.events() if ev.device_type.name == "CUDA" and "c2b_" in ev.name]
+        evs.sort(key=lambda ev: ev.time_range.start)
+        if not evs or len(evs) % args.steps:
+            raise SystemExit("kernel_times: %d kernel records for %d steps" % (len(evs), args.steps))
+        per_step = len(evs) // args.steps
+        per = defaultdict(list)
+        names = []
+        for k, ev in enumerate(evs):
+            short = ev.name.split("(")[0].replace("void ", "")
+            key = (k % per_step, short)
+            if k < per_step:
+                names.append(key)
+            per[key].append(ev.time_range.elapsed_us() / 1000.0)
+        rows = []
+        total = 0.0
+        for key in names:
+            v = per[key]
+            if len(v) != args.steps:
+                raise SystemExit("kernel_times: launch sequence differs between steps")
+            ms = sum(v) / len(v)
+            total += ms
+            rows.append({"launch": key[0] + 1, "kernel": key[1], "ms_per_launch": ms})
+        diag = route = None
         import ctypes as C
-        a, b, c = C.c_int64(), C.c_int64(), C.c_int64()
-        if L.c2b_diag_counts(eng.h, C.byref(a), C.byref(b), C.byref(c)) == 0:
-            diag = {"proved": a.value // args.steps, "tier1": b.value // args.steps, "tier2": c.value // args.steps}
+        if hasattr(L, "c2b_diag_counts"):
+            a, b, c = C.c_int64(), C.c_int64(), C.c_int64()
+            if L.c2b_diag_counts(eng.h, C.byref(a), C.byref(b), C.byref(c)) == 0:
+                diag = {"proved": a.value // args.steps, "tier1": b.value // args.steps, "tier2": c.value // args.steps}
+        if hasattr(L, "c2b_route_counts"):
+            a, b = C.c_int64(), C.c_int64()
+            if L.c2b_route_counts(eng.h, C.byref(a), C.byref(b)) == 0:
+                route = {"routed": a.value // args.steps, "kept": b.value // args.steps}
+        return rows, total, diag, route
+
+    def table(rows, total):
+        print("| # | kernel | ms / launch | share |")
+        print("|---|---|---|---|")
+        for r in rows:
+            print("| %d | %s | %.3f | %.0f %% |" % (r["launch"], r["kernel"], r["ms_per_launch"], 100.0 * r["ms_per_launch"] / total if total else 0.0))
+        print("| | sum of kernel times per step | %.3f | |" % total)
+
+    rows, total, diag, route = measure()
+    report = None
+    if args.route_report:
+        # the same steps without routing: whether a read passes the narrow tier depends on the read alone, so the narrow
+        # failures without routing (N0), the routed reads (N_r) and the narrow failures with routing (N_f) give
+        # false-narrow = N_f (kept, then failed) and false-wide = N_r - (N0 - N_f) (routed, would have passed)
+        os.environ["C2B_NO_ROUTE"] = "1"
+        try:
+            rows0, total0, diag0, _ = measure()
+        finally:
+            os.environ.pop("C2B_NO_ROUTE", None)
+        N0, Nr = diag0["tier2"], route["routed"]
+        Nf = diag["tier2"] - Nr                          # tier-2 reads = routed + narrow failures
+        report = {"listed": diag["tier1"], "N0": N0, "N_r": Nr, "N_f": Nf, "false_narrow": Nf, "false_wide": Nr - (N0 - Nf),
+                  "kernels_no_route": rows0, "total_ms_no_route": total0}
     info = card_info(0)
     print("card: %s, power limit %s W, max SM clock %s MHz" % (info.get("name"), info.get("power_limit_w"), info.get("max_sm_clock_mhz")))
     print("%d reads x 250 bp (mix %s), %d profiled steps after %d warm-up steps; C2B_NO_DIAG=%s" % (
         n, args.mix, args.steps, args.warmup, os.environ.get("C2B_NO_DIAG", "")))
-    print("| # | kernel | ms / launch | share |")
-    print("|---|---|---|---|")
-    for r in rows:
-        print("| %d | %s | %.3f | %.0f %% |" % (r["launch"], r["kernel"], r["ms_per_launch"], 100.0 * r["ms_per_launch"] / total if total else 0.0))
-    print("| | sum of kernel times per step | %.3f | |" % total)
+    table(rows, total)
     if diag is not None:
         print("reads per step: %d proved on the diagonal (%.1f %%), %d to the narrow tier, %d to the wide ring" %
               (diag["proved"], 100.0 * diag["proved"] / n, diag["tier1"], diag["tier2"]))
+    if route is not None:
+        print("routing per step: %d of the diagonal tier's unproved reads sent straight to the wide ring, %d kept for the narrow tier" %
+              (route["routed"], route["kept"]))
+    if report is not None:
+        print("\nsame steps with C2B_NO_ROUTE=1:")
+        table(report["kernels_no_route"], report["total_ms_no_route"])
+        L_ = max(report["listed"], 1)
+        print("routing report per step: listed %d, narrow failures without routing N0 = %d, routed N_r = %d, narrow failures with "
+              "routing N_f = %d; false-narrow %d (%.2f %% of listed), false-wide %d (%.2f %% of listed)" % (
+                  report["listed"], report["N0"], report["N_r"], report["N_f"], report["false_narrow"],
+                  100.0 * report["false_narrow"] / L_, report["false_wide"], 100.0 * report["false_wide"] / L_))
     if args.json:
         with open(args.json, "w") as fh:
             json.dump({"card": info, "reads": n, "steps": args.steps, "mix": args.mix, "no_diag": os.environ.get("C2B_NO_DIAG", ""),
-                       "kernels": rows, "total_ms_per_step": total, "diag_counts": diag}, fh, indent=1)
+                       "kernels": rows, "total_ms_per_step": total, "diag_counts": diag, "route_counts": route,
+                       "route_report": report}, fh, indent=1)
 
 
 if __name__ == "__main__":

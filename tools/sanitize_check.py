@@ -50,6 +50,18 @@ eng.counts_reset()
 buf, off = pack_reads(reads[:1200])
 res = eng.align_packed(buf, off, compact=True)
 print('compact+legacy', eng.path_counts(), eng.ring_counts(), res.strings_block(0, 4).shape)
+# diagonal tier with routing: bench-mix batches of 16, 17, 33 and 100 reads (partial units on the narrow and tier-2 lists),
+# routing on, off and on for every unproved read
+eng.configure({'Reference': ref}, ['Reference'], m, -20, -2, 5, 2, 0, 'ACGTN', 8)
+for sw in (None, 'C2B_NO_ROUTE', 'C2B_ROUTE_ALL'):
+    if sw:
+        os.environ[sw] = '1'
+    for nb in (16, 17, 33, 100):
+        eng.counts_reset()
+        buf, off = pack_reads(reads[:nb])
+        res = eng.align_packed(buf, off, compact=True)
+        print('route', sw, nb, eng.diag_counts(), eng.route_counts())
+    os.environ.pop(sw or 'C2B_NO_ROUTE', None)
 # FASTQ front end on the GPU: mixed line ends, blank tail, duplicates
 from crispresso2_b200 import fastq
 recs = []
