@@ -137,8 +137,8 @@ def configure_engine(engine, args, refs, ref_names, aln_matrix, edit_cap=12):
 def merge_weights(uniques, counts):
     """Weights the quantification loop ends up using after its reverse-complement merge (CRISPRessoCORE.py:3971-3975):
     walking the cache in first-seen order, a read absorbs the count of its reverse complement (which drops to 0);
-    a palindromic read absorbs itself.  Valid because a read and its reverse complement always share their aligned
-    status (same score set), so both are in the cache or neither is."""
+    a palindromic read absorbs itself.  Valid when a read and its reverse complement share their aligned status (same score
+    set), so that both are in the cache or neither is; _weights_over_aligned handles the one setting where they may not."""
     pos = {s: k for k, s in enumerate(uniques)}
     w = list(counts)
     for k, s in enumerate(uniques):
@@ -259,6 +259,22 @@ def _variant_from(res, i, seq, ref_names, refs):
 
 def res_flags(res):
     return getattr(res, "flags", 0)
+
+
+def _weights_over_aligned(engine, res, buf, off, counts, weights, args):
+    """The quantification loop merges a read with its reverse complement only when both are in variantCache, i.e. both
+    aligned (CRISPRessoCORE.py:3964-3975).  The weights passed to the batch assume a read and its reverse complement share
+    their aligned status, which holds unless --aln_seed_min is negative: then a read with no seed hit on either strand passes
+    the seed test as forward-only, and so does its reverse complement, and the two forward alignments can fall on either side
+    of min_aln_score.  -> the weights merged over the aligned reads if they differ from `weights`, else None"""
+    if args.aln_seed_min >= 0 or not len(counts):
+        return None
+    _, aligned = _serial_stats(res, counts, lib_path=engine.lib_path)
+    w = merge_weights_packed(buf, off, counts, member=aligned.astype(np.uint8), lib_path=engine.lib_path)
+    sel = aligned.astype(bool)
+    if (w[sel] == np.asarray(weights, dtype=np.int32)[sel]).all():
+        return None
+    return np.where(sel, w, np.asarray(weights, dtype=np.int32)).astype(np.int32)
 
 
 def merge_weights_packed(buf, off, counts, member=None, lib_path=None):
@@ -557,9 +573,17 @@ def _process_uniques(engine, buf, off, counts, keys, variantCache, ref_names, re
         if "err" in box:
             raise box["err"]
         res, sc_extra = box["res"], box["extra"]
+        w_aln = _weights_over_aligned(engine, res, buf_g, off_g, counts_g, weights, args)
+        if w_aln is not None:                               # the merge moved weight onto or off a read outside the cache
+            weights = w_aln
+            configure_engine(engine, args, refs, ref_names, aln_matrix)
+            engine.counts_reset()
+            res, sc_extra = _batch(engine, buf_g, off_g, counts_g, weights, ref_names, refs, flags, args, aln_matrix, scaffold)
         parts = [(0, res, _complete_edit_lists(engine, res, buf_g, off_g, flags))]
         raw = None
     else:
+        if args.aln_seed_min < 0:                           # _weights_over_aligned needs every rank's aligned status
+            raise EngineError("--aln_seed_min below 0 is not supported with several ranks (run it in one process)")
         keys, keys_g = key_lists()
         import torch.distributed as dist
         from . import dist as cdist
