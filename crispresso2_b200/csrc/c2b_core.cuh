@@ -38,8 +38,7 @@ C2B_DEV uint32_t shflu_up(uint32_t v, int d) { return __shfl_up_sync(0xffffffffu
 C2B_DEV int shfl_xor(int v, int m) { return __shfl_xor_sync(0xffffffffu, v, m); }
 C2B_DEV uint32_t ballot(bool p) { return __ballot_sync(0xffffffffu, p); }
 C2B_DEV void sync() { __syncwarp(); }
-// barrier among the g warps of this warp's phase set: named barrier 1 + set index.  g > 0: sets of g consecutive warps;
-// g < 0: |g| warps strided by the number of sets (warps w, w + nsets, ...: with four sets, the warps of one sub-partition)
+// barrier among the g warps of this warp's phase set (g consecutive warps): named barrier 1 + set index
 #ifdef C2B_X_INLINE_BARRIER
 C2B_DEV
 #else
@@ -47,10 +46,9 @@ __device__ __noinline__        // ONE barrier instruction in the binary: every w
 #endif
 void grp_sync(int g)
 {
-    // |g| and the number of sets are powers of two (checked by the host): shifts, not the integer divisions that used to
-    // be inlined at every one of the dozen phase barriers
-    const int w = (int)(threadIdx.x >> 5), n = g > 0 ? g : -g, sh = 31 - __clz(n);
-    const int set = g > 0 ? (w >> sh) : (w & (((int)(blockDim.x >> 5) >> sh) - 1));
+    // g is a power of two: shifts, not the integer divisions that used to be inlined at every one of the dozen phase barriers
+    const int w = (int)(threadIdx.x >> 5), sh = 31 - __clz(g);
+    const int set = w >> sh;
     // barrier.sync without .aligned (bar.sync is the aligned form): a warp may arrive not fully converged
     asm volatile("barrier.sync %0, %1;" ::"r"(1 + set), "r"(32 << sh) : "memory");
 }
@@ -60,6 +58,7 @@ C2B_DEV uint32_t max3_2(uint32_t a, uint32_t b, uint32_t c) { return __vimax3_s1
 C2B_DEV uint32_t addmax_2(uint32_t a, uint32_t b, uint32_t c) { return __viaddmax_s16x2(a, b, c); }  // per half max(a+b, c)
 C2B_DEV uint4 ldg4u(const uint4 *p) { return __ldg(p); }
 C2B_DEV void prefetch_l2(const void *p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
+C2B_DEV int grid_warps() { return (int)(gridDim.x * (blockDim.x >> 5)); }
 // shared-state-space accesses through a 32-bit address kept in a register (no generic-address arithmetic in hot loops)
 C2B_DEV uint32_t smem_addr(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 C2B_DEV uint32_t lds_u8(uint32_t a) { uint32_t v; asm volatile("ld.shared.u8 %0, [%1];" : "=r"(v) : "r"(a)); return v; }
@@ -89,6 +88,9 @@ C2B_DEV unsigned long long fetch_add(unsigned long long *p, unsigned long long v
 
 #else
 #include "warp_emu.h"   // provides C2B_DEV, C2B_DEVNOINL, int4/uint4 and namespace wp
+namespace wp {
+C2B_DEV int grid_warps() { return 1; }                  // the emulator runs a kernel's loop as a grid of one warp
+}  // namespace wp
 #endif
 
 namespace c2b {
@@ -141,6 +143,26 @@ constexpr int32_t RT_OFF = -(1 << 30);
 // the narrow first tier's band (align_narrow16): paths inside column - row in [-RN_DLO, RN_DHI] are computed exactly
 constexpr int RN_DLO = 17, RN_DHI = 11;
 
+// The engine's work block in device memory: what the kernels count for the host, and the hand-out counters and list lengths
+// of the launch sequence in flight.
+struct WorkBlock {
+    // cumulative path statistics (c2b_path_counts): general kernel work items through the pair path and read by read, packed
+    // pairs re-run over the full matrix; in reads: kept by the ring, sent on to the full matrix, settled by the ALIGN kernel
+    unsigned long long pair_items, single_items, band_reruns, ring_kept, ring_sent, align_settled;
+    // cumulative, the diagonal tier (c2b_diag_counts, c2b_route_counts): reads proved, put on its list, sent to the second tier
+    // (routed there or failed by the narrow tier), routed, kept for the narrow tier
+    unsigned long long diag_proved, diag_listed, tier2, routed, kept;
+    struct Launch {                        // zeroed at the start of every launch sequence
+        // work hand-out counters: ALIGN (or the general kernel alone), the second-tier ALIGN launch, the general kernel after ALIGN
+        unsigned long long align_next, tier2_next, general_next;
+        unsigned long long widest;         // widest alignment of the batch (all kernels of the launch sequence)
+        // list lengths: pairs left over for the general kernel, the tier-2 list, the narrow tier's and the diagonal tier's list
+        unsigned long long left_n, tier2_n, narrow_n, diag_n;
+    } launch;
+};
+constexpr size_t WORK_BYTES = 32 * 8;
+static_assert(sizeof(WorkBlock) <= WORK_BYTES, "work block");
+
 struct KParams {
     const uint8_t *reads; const int64_t *offsets; int64_t n_reads;
     const int32_t *count, *qweight, *ref_id;
@@ -157,26 +179,23 @@ struct KParams {
     int32_t *bnd; int64_t bnd_words_per_warp;                 // 2 x 3 x (maxJ+1): row-block boundary rows
     uint64_t *opsbuf;                                         // [warp][n_refs][32] op streams (multi-reference)
     uint64_t *rgops;                                          // [warp][RG_MAX_REFS][4 pairs][RG_OPS_STRIDE]: walked op streams of the multi-reference ring path
-    unsigned long long *work_counter;      // work hand-out counter of this launch
-    unsigned long long *widest;            // widest alignment of this batch (all kernels of the launch sequence)
+    WorkBlock *wb;
+    unsigned long long *work_counter;      // work hand-out counter of this launch (a field of wb->launch)
     // two-kernel form (c2b_split.cuh): op streams and their meta word per (read, reference) slot, written by the ALIGN kernel
     // (and by the general kernel for the pairs it aligns), read by the CLASSIFY kernel and copied out as the compact output
     uint64_t *gops; uint32_t *gmeta; int32_t NW;            // NW = W / 32 words of 32 ops per slot
-    int32_t *left; unsigned long long *left_n;              // ALIGN kernel: pairs left over for the general kernel, and their count
-    int32_t *left2; unsigned long long *left2_n;            // ALIGN kernel, narrow first tier: reads for the second-tier launch (nullptr: no narrow tier)
-    int32_t *left0; unsigned long long *left0_n;            // diagonal tier: reads it did not prove (CLASSIFY's list), and their count
-    int32_t *left1; unsigned long long *left1_n;            // diagonal tier with routing: the unproved reads it keeps for the narrow tier
+    int32_t *left;                                          // ALIGN kernel: pairs left over for the general kernel (wb->launch.left_n)
+    int32_t *left2;                                         // ALIGN kernel, narrow first tier: reads for the second-tier launch (nullptr: no narrow tier)
+    int32_t *left0;                                         // diagonal tier: reads it did not prove (CLASSIFY's list)
+    int32_t *left1;                                         // diagonal tier with routing: the unproved reads it keeps for the narrow tier
     int32_t route;                                          // diagonal tier: 0 no routing, 1 route_read decides, 2 route every unproved read
-    unsigned long long *diag_n;                             // diagonal tier: [0] reads proved, [1] reads put on its list, [2] tier-2 reads, [3] routed, [4] kept (cumulative)
-    const unsigned long long *n_dev;                        // general kernel over the left-over list: *n_dev reads (entries of pair_order)
-    int32_t discard_slab;                                   // ALIGN kernel: drop the dead slab lines from L2 instead of writing them back
-    unsigned long long *stats;             // cumulative path statistics (c2b_path_counts), indices 2..7; [26] reads sent to the second tier
+    const unsigned long long *n_dev;                        // launch over a list: *n_dev reads (entries of pair_order)
     int32_t vstride, hstride;
     const uint32_t *stage_src;        // = refs[0].prof2 (global source of the staged tile)
     int32_t stage_bytes;              // bytes of refs[0].prof2 staged into shared memory by TMA at kernel start (0: none)
     const uint8_t *lut;               // [256] ASCII -> alphabet code, 255 = not in the alphabet (device memory, L1-resident)
     int32_t phase_sync;               // g > 0: sets of g consecutive warps of a CTA walk through the per-group phases in step
-                                      // (instruction-cache locality; g divides the CTA's warp count); 0: free-running warps
+                                      // (instruction-cache locality; a power of two dividing the CTA's warp count); 0: free-running warps
     const uint64_t *forced_ops;       // c2b_classify_aligned: op streams supplied by the caller, [read][32]
     const int32_t *forced_n;
 };
@@ -1114,7 +1133,7 @@ C2B_DEV void process_read(const KParams &P, WarpSmem &S, int64_t rd, int warp_sl
                     if (lane < P.NW) P.gops[oslot(P, rd, r) * P.NW + lane] = wk.ops;
                     if (lane == 0) P.gmeta[oslot(P, rd, r)] = (uint32_t)wk.n | ((uint32_t)use_rc << 16) | (2u << 24);
                 }
-                if (lane == 0) wp::maxg(P.widest, (unsigned long long)wk.n);   // widest alignment of the launch
+                if (lane == 0) wp::maxg(&P.wb->launch.widest, (unsigned long long)wk.n);   // widest alignment of the launch
                 keep_irr = co.irregular;
                 note_score(rec, R, r, a.score_milli);
             }
@@ -1247,7 +1266,7 @@ C2B_DEV Walked align_pair(const KParams &P, const RefDev &R, const uint32_t *pro
         const Walked wk = walk_batch<true>(P, R, J, reinterpret_cast<const uint32_t *>(tb2), s, sm);
         if (!band || !wp::ballot((wk.err & 4) != 0)) return wk;
         band = false;                                               // a traceback left the band: once more with the full slab
-        if (wp::lane() == 0) wp::addg(P.stats + 4, 1);
+        if (wp::lane() == 0) wp::addg(&P.wb->band_reruns, 1);
     }
 }
 
@@ -1474,7 +1493,7 @@ C2B_DEVNOINL void process_pair(const KParams &P, WarpSmem &S, const uint32_t *st
             a.irregular_ends = (uint8_t)co.irregular;
             keep_irr = co.irregular;
             note_score(rec, R, r, a.score_milli);
-            if (hl == 0) wp::maxg(P.widest, (unsigned long long)bn);
+            if (hl == 0) wp::maxg(&P.wb->launch.widest, (unsigned long long)bn);
         }
         if (multi) opsbuf[r * 32 + lane] = bops;
         if (P.gops && !a.status && (h == 0 || rdB != rdA)) {
@@ -1528,7 +1547,7 @@ C2B_DEV void process_item(const KParams &P, WarpSmem &S, const uint32_t *staged_
             for (int r = r_begin; r < r_end; r++) if (Ja > refdev(P, r).pk_maxJ || refdev(P, r).I + Ja > PK_MAX_ALN) pair = false;
         }
     }
-    if (wp::lane() == 0) wp::addg(P.stats + (pair ? 2 : 3), 1);      // path statistics (c2b_path_counts)
+    if (wp::lane() == 0) wp::addg(pair ? &P.wb->pair_items : &P.wb->single_items, 1);      // path statistics (c2b_path_counts)
     if (pair) process_pair<ONE>(P, S, staged_prof, rdA, rdB, warp_slot, nullptr, false);
     else {
         process_read<ONE>(P, S, rdA, warp_slot);
@@ -1608,9 +1627,9 @@ C2B_DEV void process_quad(const KParams &P, WarpSmem &S, QuadSmem &Q, const uint
     }
     wp::sync();
     if (lane == 0) {
-        wp::addg(P.stats + 2, 4);
-        wp::addg(P.stats + 5, 2 * wp::popc(passmask));            // [5], [6]: in reads (the host reports pairs)
-        wp::addg(P.stats + 6, 2 * (4 - wp::popc(passmask)));
+        wp::addg(&P.wb->pair_items, 4);
+        wp::addg(&P.wb->ring_kept, 2 * wp::popc(passmask));       // in reads (the host reports pairs)
+        wp::addg(&P.wb->ring_sent, 2 * (4 - wp::popc(passmask)));
     }
 #pragma unroll 1
     for (int q = 0; q < 4; q++) {
@@ -1702,9 +1721,9 @@ C2B_DEVNOINL void process_quad_multi(const KParams &P, WarpSmem &S, QuadSmem &Q,
     }
     if (P.phase_sync) wp::grp_sync(P.phase_sync);
     if (lane == 0) {
-        wp::addg(P.stats + 2, 4);
-        wp::addg(P.stats + 5, 2 * npass);
-        wp::addg(P.stats + 6, 2 * (4 * P.n_refs - npass));
+        wp::addg(&P.wb->pair_items, 4);
+        wp::addg(&P.wb->ring_kept, 2 * npass);
+        wp::addg(&P.wb->ring_sent, 2 * (4 * P.n_refs - npass));
     }
 #pragma unroll 1
     for (int q = 0; q < 4; q++) {
@@ -1753,6 +1772,22 @@ C2B_DEV void process_group(const KParams &P, WarpSmem &S, QuadSmem &Q, const uin
 #pragma unroll 1
             for (int b = group_phases(P); b > 0; b--) wp::grp_sync(P.phase_sync);
         }
+    }
+}
+
+// The general kernel's loop over the ALIGN kernel's left-over list (P.pair_order, *P.n_dev entries): one pair per hand-out (a
+// warp that drew four hard pairs in a row was the critical path of the whole launch).  `warp` names the warp's scratch slabs.
+template <bool ONE>
+C2B_DEV void general_list_loop(const KParams &P, WarpSmem &S, const uint32_t *staged_prof, int warp)
+{
+    const unsigned total = (unsigned)((nreads(P) + 1) / 2);
+    for (;;) {
+        unsigned w = 0;
+        if (wp::lane() == 0) w = (unsigned)wp::fetch_work(P.work_counter);
+        w = (unsigned)wp::shfl((int)w, 0);
+        if (w >= total) break;
+        process_item<ONE>(P, S, staged_prof, (int64_t)w, warp);
+        wp::sync();
     }
 }
 

@@ -125,14 +125,14 @@ static void rt_host_free(void *p) { free(p); }
 #endif
 
 // ----------------------------------------------------------------------------------------- kernel
-#ifndef C2B_EMU
 #ifndef C2B_WARPS_PER_CTA
 #define C2B_WARPS_PER_CTA 8
 #endif
 #ifndef C2B_MIN_CTAS_PER_SM
 #define C2B_MIN_CTAS_PER_SM 2
 #endif
-constexpr int WARPS_PER_CTA = C2B_WARPS_PER_CTA;      // launch-bounds maximum; the launch may use fewer (env C2B_WARPS_PER_CTA)
+constexpr int WARPS_PER_CTA = C2B_WARPS_PER_CTA;      // general and ALIGN kernels
+static_assert(WARPS_PER_CTA % 4 == 0, "the general kernel's phase sets are four warps");
 #ifndef C2B_B_WARPS
 #define C2B_B_WARPS 4
 #endif
@@ -140,7 +140,12 @@ constexpr int B_WARPS_PER_CTA = C2B_B_WARPS;                    // CLASSIFY kern
 #ifndef C2B_B_MIN_CTAS
 #define C2B_B_MIN_CTAS 6
 #endif
+#ifndef C2B_A_MIN_CTAS
+#define C2B_A_MIN_CTAS 2
+#endif
+constexpr int D_WARPS_PER_CTA = 8;                               // diagonal tier
 
+#ifndef C2B_EMU
 // TMA-staged reference tile: the packed substitution profile of reference 0, once per CTA (cp.async.bulk + mbarrier);
 // every DP step then reads it with two 16-byte LDS.  -> shared-memory address of the tile, or nullptr
 __device__ __forceinline__ const uint32_t *stage_profile(const KParams &P, unsigned char *dst)
@@ -162,6 +167,9 @@ __device__ __forceinline__ const uint32_t *stage_profile(const KParams &P, unsig
     return reinterpret_cast<const uint32_t *>(dst);
 }
 
+// Each kernel carves up its shared memory, stages the profile tile and runs its loop (c2b_split.cuh, c2b_core.cuh); the
+// emulator build runs the same loops as a grid of one warp (run_plan).
+
 // GENERAL kernel: the whole per-read path in one launch (any length within the build limits, any parameters; full-matrix
 // DP paths of c2b_core.cuh).  Since r02 it runs after the ALIGN / CLASSIFY pair, over the pairs ALIGN left over (P.n_dev,
 // P.pair_order = the left-over list), or alone when the two-kernel form does not apply.
@@ -176,27 +184,19 @@ __global__ void __launch_bounds__(WARPS_PER_CTA * 32, C2B_MIN_CTAS_PER_SM) c2b_a
     QuadSmem *Q = reinterpret_cast<QuadSmem *>(smem_raw + (size_t)(blockDim.x >> 5) * sizeof(WarpSmem)) + (threadIdx.x >> 5);
     const int warp_slot = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     const uint32_t *staged_prof = stage_profile(P, smem_raw + (((size_t)(blockDim.x >> 5) * (sizeof(WarpSmem) + sizeof(QuadSmem)) + 127) & ~(size_t)127));
-    // Work groups (8 reads each) are handed out per phase set (g consecutive warps, one group per warp), one hand-out
-    // ahead, so that the loop count -- and with it the number of barriers executed by process_group's phases -- is the
-    // same for every warp of the set, and the next group's read bytes are on their way to L2 while this one computes.
-    __shared__ unsigned long long next_base[WARPS_PER_CTA];
-    const int gs = P.phase_sync, g = gs > 0 ? gs : gs < 0 ? -gs : 1, wib = threadIdx.x >> 5, nsets = (int)(blockDim.x >> 5) / g;
-    const int set = gs < 0 ? wib % nsets : wib / g, wis = gs < 0 ? wib / nsets : wib % g;
-    const int64_t nrd = nreads(P);
     if (P.n_dev) {
-        // over the ALIGN kernel's left-over list: one pair per hand-out (a warp that drew four hard pairs in a row was the
-        // critical path of the whole launch)
-        const unsigned total = (unsigned)((nrd + 1) / 2);
-        for (;;) {
-            unsigned w = 0;
-            if ((threadIdx.x & 31) == 0) w = (unsigned)atomicAdd(P.work_counter, 1ull);
-            w = __shfl_sync(0xffffffffu, w, 0);
-            if (w >= total) break;
-            process_item<ONE>(P, *S, staged_prof, (int64_t)w, warp_slot);
-            __syncwarp();
-        }
+        general_list_loop<ONE>(P, *S, staged_prof, warp_slot);
         return;
     }
+    // Phase sets: work groups (8 reads each) are handed out per set of g consecutive warps, one group per warp, one hand-out
+    // ahead, so that the loop count -- and with it the number of barriers executed by process_group's phases -- is the same
+    // for every warp of the set, and the next group's read bytes are on their way to L2 while this one computes.  This loop
+    // needs the warps of a set in step, so it is the one loop the emulator does not share: it runs process_group per group
+    // there and checks the barrier count of each (run_plan).
+    __shared__ unsigned long long next_base[WARPS_PER_CTA];
+    const int gs = P.phase_sync, g = gs > 0 ? gs : 1, wib = threadIdx.x >> 5;
+    const int set = wib / g, wis = wib % g;
+    const int64_t nrd = nreads(P);
     const unsigned long long total = ((unsigned long long)nrd + 7) / 8;
     auto hand_out = [&]() -> unsigned long long {
         if (wis == 0 && (threadIdx.x & 31) == 0) next_base[set] = atomicAdd(P.work_counter, (unsigned long long)g);
@@ -223,134 +223,29 @@ __global__ void __launch_bounds__(WARPS_PER_CTA * 32, C2B_MIN_CTAS_PER_SM) c2b_a
     }
 }
 
-// ALIGN kernel (c2b_split.cuh: align_group): persistent, free-running warps pull work groups of 8 reads from a counter.
-#ifndef C2B_A_MIN_CTAS
-#define C2B_A_MIN_CTAS 2
-#endif
+// ALIGN kernel (c2b_split.cuh: align_loop)
 __global__ void __launch_bounds__(WARPS_PER_CTA * 32, C2B_A_MIN_CTAS) c2b_align_kernel(const __grid_constant__ KParams P)
 {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     ASmem *S = reinterpret_cast<ASmem *>(smem_raw) + (threadIdx.x >> 5);
     const int nw = blockDim.x >> 5;
-    const int warp_slot = blockIdx.x * nw + (threadIdx.x >> 5);
     const uint32_t *staged_prof = stage_profile(P, smem_raw + (((size_t)nw * sizeof(ASmem) + 127) & ~(size_t)127));
-    asmem_init(P, *S);
-    const int64_t nrd = nreads(P);
-    const unsigned ahead = gridDim.x * nw;
-    if (P.left2) {
-        // narrow first tier: work in units of sixteen reads; units it does not take run as two ordinary groups of eight
-        const unsigned total = (unsigned)((nrd + 15) / 16);
-        for (;;) {
-            unsigned w = 0;
-            if ((threadIdx.x & 31) == 0) w = (unsigned)atomicAdd(P.work_counter, 1ull);
-            w = __shfl_sync(0xffffffffu, w, 0);
-            if (w >= total) break;
-            if (w + ahead < total) {                            // the unit this warp is likely to get next: bytes towards L2
-                const int64_t g = (int64_t)w + ahead;
-                if (!P.pair_order) {
-                    const int64_t last = 16 * g + 16 < nrd ? 16 * g + 16 : nrd;
-                    const int64_t a = P.offsets[16 * g] + (int64_t)(threadIdx.x & 31) * 128;
-                    if (a < P.offsets[last]) asm volatile("prefetch.global.L2 [%0];" ::"l"(P.reads + a));
-                } else {                                        // reads of the diagonal tier's list: two lanes per read
-                    const int64_t x = 16 * g + ((threadIdx.x & 31) >> 1);
-                    if (x < nrd) {
-                        const int64_t rd = read_at(P, x);
-                        const int64_t b1 = P.offsets[rd + 1];
-                        for (int64_t a = (P.offsets[rd] & ~(int64_t)127) + (int64_t)(threadIdx.x & 1) * 128; a < b1; a += 256)
-                            asm volatile("prefetch.global.L2 [%0];" ::"l"(P.reads + a));
-                    }
-                }
-            }
-            if (!align_narrow16(P, *S, staged_prof, (int64_t)w, warp_slot)) {
-                align_group(P, *S, staged_prof, 2 * (int64_t)w, warp_slot);
-                __syncwarp();
-                if (8 * (2 * (int64_t)w + 1) < nrd) align_group(P, *S, staged_prof, 2 * (int64_t)w + 1, warp_slot);
-            }
-            __syncwarp();
-        }
-        return;
-    }
-    const unsigned total = (unsigned)((nrd + 7) / 8);
-    for (;;) {
-        unsigned w = 0;
-        if ((threadIdx.x & 31) == 0) w = (unsigned)atomicAdd(P.work_counter, 1ull);
-        w = __shfl_sync(0xffffffffu, w, 0);
-        if (w >= total) break;
-        if (w + ahead < total && !P.pair_order) {           // the group this warp is likely to get next: bytes towards L2
-            const int64_t g = (int64_t)w + ahead;
-            const int64_t last = 8 * g + 8 < nrd ? 8 * g + 8 : nrd;
-            const int64_t a = P.offsets[8 * g] + (int64_t)(threadIdx.x & 31) * 128;
-            if (a < P.offsets[last]) asm volatile("prefetch.global.L2 [%0];" ::"l"(P.reads + a));
-        }
-        align_group(P, *S, staged_prof, (int64_t)w, warp_slot);
-        __syncwarp();
-    }
+    align_loop(P, *S, staged_prof, blockIdx.x * nw + (threadIdx.x >> 5));
 }
 
-// Diagonal tier (c2b_split.cuh: diag_unit): one read per warp, units of 32 consecutive reads strided over the grid.
-constexpr int D_WARPS_PER_CTA = 8;
+// Diagonal tier (c2b_split.cuh: diag_loop)
 __global__ void __launch_bounds__(D_WARPS_PER_CTA * 32) c2b_diag_kernel(const __grid_constant__ KParams P)
 {
     __shared__ DSmem smem[D_WARPS_PER_CTA];
-    DSmem &S = smem[threadIdx.x >> 5];
-    dsmem_init(P, S);
-    ScAcc<1> acc;
-    sc_init(acc);
-    const int64_t units = (P.n_reads + 31) / 32;
-    int proved = 0, seen = 0, routed = 0;
-    for (int64_t u = (int64_t)blockIdx.x * D_WARPS_PER_CTA + (threadIdx.x >> 5); u < units; u += (int64_t)gridDim.x * D_WARPS_PER_CTA) {
-        int k = 0;
-        proved += diag_unit(P, S, u, acc, k);
-        routed += k;
-        seen += P.n_reads - 32 * u < 32 ? (int)(P.n_reads - 32 * u) : 32;
-        __syncwarp();
-    }
-    sc_flush(acc, P);
-    if ((threadIdx.x & 31) == 0 && seen) {
-        wp::addg(P.diag_n, proved); wp::addg(P.diag_n + 1, seen - proved);
-        wp::addg(P.diag_n + 2, routed);                  // tier-2 reads: routed here, and the narrow tier's failures
-        wp::addg(P.diag_n + 3, routed); wp::addg(P.diag_n + 4, seen - proved - routed);
-    }
+    diag_loop(P, smem[threadIdx.x >> 5], (int64_t)blockIdx.x * D_WARPS_PER_CTA + (threadIdx.x >> 5), (int64_t)gridDim.x * D_WARPS_PER_CTA);
 }
 
-// CLASSIFY kernel (c2b_split.cuh: classify_read): one aligned read per warp, reads strided over the grid -- every read, or
-// (after the diagonal tier, which classifies the reads it proves) the entries of its list: P.pair_order, *P.n_dev of them.
+// CLASSIFY kernel (c2b_split.cuh: classify_loop)
 template <bool ONE>
 __global__ void __launch_bounds__(B_WARPS_PER_CTA * 32, C2B_B_MIN_CTAS) c2b_classify_kernel(const __grid_constant__ KParams P)
 {
     __shared__ BSmem smem[B_WARPS_PER_CTA];
-    BSmem &S = smem[threadIdx.x >> 5];
-    const int64_t nw = (int64_t)gridDim.x * B_WARPS_PER_CTA;
-    const int64_t total_bytes = P.offsets[P.n_reads];
-    const int64_t n = nreads(P);
-    int64_t x = (int64_t)blockIdx.x * B_WARPS_PER_CTA + (threadIdx.x >> 5);      // position in the read order
-    if (x >= n) return;
-    ScAcc<ONE ? 1 : RG_MAX_REFS> acc;
-    sc_init(acc);
-    // two-deep input pipeline: stage A of position x + 2 nw and stage B of x + nw are in flight while x is classified; the
-    // read at x + 3 nw is looked up one iteration before its stage A needs it (a list entry, then its offsets: two round trips)
-    int32_t rd = (int32_t)read_at(P, x), rd1 = 0, rd2 = 0;
-    BPreA a1 = classify_pre_a(P, rd);
-    BPre pre = classify_pre_b<ONE>(P, rd, a1, total_bytes);
-    if (x + nw < n) { rd1 = (int32_t)read_at(P, x + nw); a1 = classify_pre_a(P, rd1); }
-    if (x + 2 * nw < n) rd2 = (int32_t)read_at(P, x + 2 * nw);
-    while (x < n) {
-        const BPre cur = pre;
-        const int32_t rc = rd;
-        if (cur.go) classify_stage<ONE>(cur, S);
-        __syncwarp();
-        const int64_t nxt = x + nw;
-        if (nxt < n) {
-            pre = classify_pre_b<ONE>(P, rd1, a1, total_bytes);
-            rd = rd1;
-            if (nxt + nw < n) { a1 = classify_pre_a(P, rd2); rd1 = rd2; }
-            if (nxt + 2 * nw < n) rd2 = (int32_t)read_at(P, nxt + 2 * nw);
-        }
-        if (cur.go) classify_read<ONE>(P, rc, cur, S, acc);
-        __syncwarp();
-        x = nxt;
-    }
-    sc_flush(acc, P);
+    classify_loop<ONE>(P, smem[threadIdx.x >> 5], (int64_t)blockIdx.x * B_WARPS_PER_CTA + (threadIdx.x >> 5), (int64_t)gridDim.x * B_WARPS_PER_CTA);
 }
 #endif
 
@@ -379,7 +274,7 @@ struct c2b_engine {
     // scratch
     DevBuf tb, tbb, tbq, bnd, ops, rgo, work, lut;
     DevBuf gops, gmeta, left, left2, left0, left1;   // device-pointer API: op streams / meta words / left-over lists of the last launch
-    int n_warps = 0, grid = 0, wpc = 8, stage_cap = 0;
+    int n_warps = 0, grid = 0, stage_cap = 0;
     int grid_a = 0, grid_b = 0, stage_cap_a = 0;       // ALIGN / CLASSIFY kernels
     int split_ok = 0, split_all = 0;                   // configuration admits the two-kernel form (some / all references)
     int diag_any = 0;                                  // some reference admits the diagonal tier (RefDev::dg_ok)
@@ -392,10 +287,7 @@ struct c2b_engine {
                    uint8_t *h_in = nullptr, *h_out = nullptr; size_t h_in_cap = 0, h_out_cap = 0;
                    int64_t d_c0 = 0, d_n = 0; size_t d_Wt = 0; bool drain = false;     // chunk waiting in h_out
                    rt_event in_done, k_done, out_done; bool used = false; } stage[2];
-    rt_stream s_in = 0, s_out = 0, stream2 = 0;     // stream2: second compute stream, kernels of odd chunks
-    rt_event fork_ev = 0;                           // orders stream2 after what is already queued on `stream`
-    size_t set_tb = 0, set_tbb = 0, set_tbq = 0, set_bnd = 0, set_ops = 0, set_rgo = 0;   // bytes per scratch set (two sets: kernels of
-                                                    // consecutive chunks overlap their tail / head on the two streams)
+    rt_stream s_in = 0, s_out = 0;
     bool pipe_ready = false;
     double last_ms = 0; int64_t launches = 0;
     const uint64_t *forced_ops = nullptr; const int32_t *forced_n = nullptr;
@@ -481,8 +373,6 @@ int c2b_create(int device, c2b_engine **out)
     cudaError_t r = cudaSetDevice(device);
     if (r == cudaSuccess) e->numa_node = numa_bind_for_device(device);
     if (r == cudaSuccess) r = cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking);
-    if (r == cudaSuccess) r = cudaStreamCreateWithFlags(&e->stream2, cudaStreamNonBlocking);
-    if (r == cudaSuccess) r = cudaEventCreateWithFlags(&e->fork_ev, cudaEventDisableTiming);
     if (r == cudaSuccess) r = cudaEventCreate(&e->ev0);
     if (r == cudaSuccess) r = cudaEventCreate(&e->ev1);
     int nsm = 0, occ = 0, smem_sm = 0, optin = 0;
@@ -511,7 +401,7 @@ int c2b_create(int device, c2b_engine **out)
             occ = std::min(occ, o);
         }
     }
-    // ALIGN kernel: its own (smaller) per-warp state; CTAs per SM from the occupancy query, optionally capped (C2B_A_CTAS_PER_SM)
+    // ALIGN kernel: its own (smaller) per-warp state; CTAs per SM from the occupancy query
     int occ_a = 0, occ_b = 0;
     e->stage_cap_a = tile_room(sizeof(ASmem), C2B_A_MIN_CTAS);
     const int dyn_a = (int)(sizeof(ASmem) * WARPS_PER_CTA) + 128 + e->stage_cap_a;
@@ -527,17 +417,13 @@ int c2b_create(int device, c2b_engine **out)
     if (occ < 1) occ = 1;
     if (occ_a < 1) occ_a = 1;
     if (occ_b < 1) occ_b = 1;
-    if (occ < C2B_MIN_CTAS_PER_SM && !getenv("C2B_CTAS_PER_SM"))
+    if (occ < C2B_MIN_CTAS_PER_SM)
         fprintf(stderr, "[c2b] warning: only %d CTA(s) of the general kernel fit an SM (built for %d)\n", occ, C2B_MIN_CTAS_PER_SM);
-    e->wpc = WARPS_PER_CTA;
-    if (const char *v = getenv("C2B_WARPS_PER_CTA")) { int k = atoi(v); if (k >= 1 && k <= WARPS_PER_CTA) e->wpc = k; }
-    if (const char *v = getenv("C2B_CTAS_PER_SM")) { int k = atoi(v); if (k >= 1 && k <= occ) occ = k; }
-    if (const char *v = getenv("C2B_A_CTAS_PER_SM")) { int k = atoi(v); if (k >= 1 && k <= occ_a) occ_a = k; }
     if (occ_a > C2B_A_MIN_CTAS) occ_a = C2B_A_MIN_CTAS;
     e->grid = nsm * occ;                 // persistent: one wave of CTAs, warps pull work items from a counter
     e->grid_a = nsm * occ_a;
     e->grid_b = nsm * std::min(occ_b, 8);
-    e->n_warps = std::max(e->grid, e->grid_a) * e->wpc;  // scratch slabs are per resident warp of whichever kernel is larger
+    e->n_warps = std::max(e->grid, e->grid_a) * WARPS_PER_CTA;  // scratch slabs are per resident warp of whichever kernel is larger
     if (getenv("C2B_VERBOSE"))
         fprintf(stderr, "[c2b] device %d (NUMA node %d): general kernel %d CTAs/SM, ALIGN %d CTAs/SM (tile room %d B), CLASSIFY %d CTAs/SM x %d warps\n",
                 device, e->numa_node, occ, occ_a, e->stage_cap_a, std::min(occ_b, 8), B_WARPS_PER_CTA);
@@ -569,8 +455,6 @@ void c2b_destroy(c2b_engine *e)
     if (e->ev0) cudaEventDestroy(e->ev0);
     if (e->ev1) cudaEventDestroy(e->ev1);
     if (e->stream) cudaStreamDestroy(e->stream);
-    if (e->stream2) cudaStreamDestroy(e->stream2);
-    if (e->fork_ev) cudaEventDestroy(e->fork_ev);
 #endif
     delete e;
 }
@@ -858,63 +742,22 @@ int c2b_string_width(const c2b_engine *e, int32_t max_read_len)
     return (e->max_I + max_read_len + 31) & ~31;
 }
 
-// work block (u64): [2..7] cumulative path statistics, [24..26] the diagonal tier's (c2b_diag_counts), [27..28] its routing
-// (c2b_route_counts); set s: [8 + 8 s] work hand-out counter, [9 + 8 s] widest alignment, [13 + 8 s] length of the tier-2
-// list, [14 + 8 s] of the narrow tier's list, [15 + 8 s] of the diagonal tier's list
-constexpr size_t WORK_BYTES = 32 * 8;
-
 static int ensure_scratch(c2b_engine *e, int maxJ)
 {
     const int TS = ((maxJ + 32 + 31) & ~31);
     if (TS <= e->scratch_TS) return C2B_OK;
     int rc;
     auto al = [](size_t x) { return (x + 255) & ~(size_t)255; };
-    e->set_tb = al((size_t)e->n_warps * e->max_nrb * TS * 64 * 4);      // 64: a pair stores two words per lane
-    e->set_tbb = al((size_t)e->n_warps * PK_BAND_SLOTS * 64 * 4);        // banded slabs (packed path)
-    e->set_tbq = al((size_t)e->n_warps * TS * 64 * 4 + 64);              // ring-banded path: (step, lane) entries
-    e->set_bnd = al((size_t)e->n_warps * 2 * 3 * TS * 4);
-    e->set_ops = al((size_t)e->n_warps * std::min(e->n_refs, (int)C2B_MAX_REFS) * 32 * 8);
-    if ((rc = ensure(e, e->tb, 2 * e->set_tb))) return rc;
-    if ((rc = ensure(e, e->tbb, 2 * e->set_tbb))) return rc;
-    if ((rc = ensure(e, e->tbq, 2 * e->set_tbq))) return rc;
-    if ((rc = ensure(e, e->bnd, 2 * e->set_bnd))) return rc;
-    if ((rc = ensure(e, e->ops, 2 * e->set_ops))) return rc;
-    e->set_rgo = al((size_t)e->n_warps * RG_MAX_REFS * 4 * RG_OPS_STRIDE * 8);
-    if ((rc = ensure(e, e->rgo, 2 * e->set_rgo))) return rc;
+    if ((rc = ensure(e, e->tb, al((size_t)e->n_warps * e->max_nrb * TS * 64 * 4)))) return rc;      // 64: a pair stores two words per lane
+    if ((rc = ensure(e, e->tbb, al((size_t)e->n_warps * PK_BAND_SLOTS * 64 * 4)))) return rc;        // banded slabs (packed path)
+    if ((rc = ensure(e, e->tbq, al((size_t)e->n_warps * TS * 64 * 4 + 64)))) return rc;              // ring-banded path: (step, lane) entries
+    if ((rc = ensure(e, e->bnd, al((size_t)e->n_warps * 2 * 3 * TS * 4)))) return rc;
+    if ((rc = ensure(e, e->ops, al((size_t)e->n_warps * std::min(e->n_refs, (int)C2B_MAX_REFS) * 32 * 8)))) return rc;
+    if ((rc = ensure(e, e->rgo, al((size_t)e->n_warps * RG_MAX_REFS * 4 * RG_OPS_STRIDE * 8)))) return rc;
     const bool fresh_work = !e->work.p;
     if ((rc = ensure(e, e->work, WORK_BYTES))) return rc;
     if (fresh_work) RTCHK(rt_zero(e->work.p, WORK_BYTES, e->stream));
     e->scratch_TS = TS;
-#ifndef C2B_EMU
-    {   // L2 policy for the traceback slabs (written once, read back by the same warp microseconds later).  C2B_L2_PERSIST:
-        //   unset / "none": no set-aside -- the whole L2 serves every access (r02 default: the ALIGN kernel's ring slabs are
-        //                   the hot set now, and a set-aside sized for the general kernel's banded slabs took 60 % of L2 away);
-        //   "ring"        : persisting window over the ring slabs (hit ratio = set-aside / slab bytes);
-        //   "band"        : the r01 setting, persisting window over the general kernel's banded slabs.
-        cudaDeviceProp prop;
-        const char *mode = getenv("C2B_L2_PERSIST");
-        if (cudaGetDeviceProperties(&prop, e->device) == cudaSuccess && prop.persistingL2CacheMaxSize > 0) {
-            cudaStreamAttrValue av; memset(&av, 0, sizeof av);
-            size_t carve = 0;
-            if (mode && (!strcmp(mode, "ring") || !strcmp(mode, "band"))) {
-                const bool ring = !strcmp(mode, "ring");
-                const size_t slab = ring ? e->set_tbq : 2 * e->set_tbb;
-                carve = std::min((size_t)prop.persistingL2CacheMaxSize, slab);
-                av.accessPolicyWindow.base_ptr = ring ? e->tbq.p : e->tbb.p;
-                av.accessPolicyWindow.num_bytes = std::min(slab, (size_t)prop.accessPolicyMaxWindowSize);
-                av.accessPolicyWindow.hitRatio = (float)std::min(1.0, (double)carve / (double)std::max<size_t>(1, av.accessPolicyWindow.num_bytes));
-                av.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
-                av.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
-            }
-            cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, carve);
-            cudaStreamSetAttribute(e->stream, cudaStreamAttributeAccessPolicyWindow, &av);
-            cudaGetLastError();
-            if (getenv("C2B_VERBOSE"))
-                fprintf(stderr, "[c2b] scratch for %d warps: ring slabs %.1f MB, L2 %.1f MB, persisting set-aside %.1f MB (%s)\n",
-                        e->n_warps, e->set_tbq / 1e6, prop.l2CacheSize / 1e6, carve / 1e6, mode ? mode : "none");
-        }
-    }
-#endif
     return C2B_OK;
 }
 
@@ -936,210 +779,200 @@ static int score_range_ok(c2b_engine *e, int64_t maxJ, const char *who)
     return C2B_OK;
 }
 
-// One batch on compute stream `cs` using scratch set `set` (0 or 1): the ALIGN / CLASSIFY pair followed by the general
-// kernel over what ALIGN left over -- or the general kernel alone where the two-kernel form does not apply.  Launches that
-// may overlap in time must use different sets; launches on the same stream are ordered.
-// d_gops / d_gmeta / d_left: op streams [n_reads * R * W/32] u64, meta words [n_reads * R], left-over list [n_reads + 8] i32;
-// d_left2 / d_left0 / d_left1: the tier-2 list, the diagonal tier's list and the narrow tier's list after routing, each
-// [n_reads + 16] i32 (nullptr: that tier / routing is off).
-static int launch_on(c2b_engine *e, rt_stream cs, int set, const uint8_t *d_reads, const int64_t *d_offsets, int64_t n_reads,
-                     int32_t max_read_len, const int32_t *d_count, const int32_t *d_qweight,
-                     const int32_t *d_ref_id, c2b_read_rec *d_recs, c2b_aln_rec *d_alns,
-                     uint8_t *d_strings, c2b_edit *d_edits, uint64_t *d_gops, uint32_t *d_gmeta, int32_t *d_left, int32_t *d_left2 = nullptr,
-                     int32_t *d_left0 = nullptr, int32_t *d_left1 = nullptr)
+// One batch's device arrays.  gops / gmeta / left: op streams [n_reads * R * W/32] u64, meta words [n_reads * R], left-over
+// list [n_reads + 8] i32; left2 / left0 / left1: the tier-2 list, the diagonal tier's list and the narrow tier's list after
+// routing, each [n_reads + 16] i32 (nullptr: that tier / routing is off).
+struct Batch {
+    const uint8_t *reads; const int64_t *offsets; int64_t n_reads; int32_t max_read_len;
+    const int32_t *count, *qweight, *ref_id;
+    c2b_read_rec *recs; c2b_aln_rec *alns; uint8_t *strings; c2b_edit *edits;
+    uint64_t *gops; uint32_t *gmeta; int32_t *left, *left2, *left0, *left1;
+};
+
+// Launch switches, read once per batch (tests toggle them between batches on one engine): the launch sequence without the
+// diagonal tier, without its routing, with every unproved read routed, without the narrow first tier, the general kernel alone.
+struct Switches { bool no_diag, no_route, route_all, no_narrow, no_split; };
+static Switches read_switches()
 {
-    if (!e || !e->configured) return fail(e, C2B_E_STATE, "c2b_align_batch: engine not configured");
-    if (n_reads < 0 || !d_recs || !d_alns || (n_reads && (!d_reads || !d_offsets))) return fail(e, C2B_E_ARG, "c2b_align_batch: bad argument");
-    if (n_reads >= (1ll << 31)) return fail(e, C2B_E_LIMIT, "c2b_align_batch: more than 2^31 reads in one batch");
-    if (max_read_len < 1) max_read_len = 1;
-    if (max_read_len > C2B_MAX_READ_LEN) return fail(e, C2B_E_LIMIT, "c2b_align_batch: read longer than C2B_MAX_READ_LEN");
-    if ((int64_t)std::abs((long long)e->prm.gap_open) * max_read_len * e->max_I >= (1ll << 28))
-        return fail(e, C2B_E_LIMIT, "c2b_align_batch: gap_open * lengths exceeds the int32 score range");
-    if (int rc0 = score_range_ok(e, max_read_len, "c2b_align_batch")) return rc0;
-    if (!d_ref_id && e->n_refs > C2B_MAX_REFS)
-        return fail(e, C2B_E_LIMIT, "c2b_align_batch: more than C2B_MAX_REFS references need a per-read ref_id");
-    int rc = ensure_scratch(e, max_read_len);
-    if (rc) return rc;
-    if (n_reads == 0) return C2B_OK;
+    return {getenv("C2B_NO_DIAG") != nullptr, getenv("C2B_NO_ROUTE") != nullptr, getenv("C2B_ROUTE_ALL") != nullptr,
+            getenv("C2B_NO_NARROW") != nullptr, getenv("C2B_NO_SPLIT") != nullptr};
+}
+
+// A batch's launch sequence: the kernels in order, each with its parameters and launch geometry.
+enum StepKind { STEP_DIAG, STEP_ALIGN, STEP_CLASSIFY, STEP_GENERAL };
+struct Step { StepKind kind; KParams P; int grid, block; size_t smem; };
+struct Plan { Step step[5]; int n = 0; bool one = false; };      // one: CLASSIFY / GENERAL in their one-candidate form
+
+// The only place that decides a batch's launch sequence: the two-kernel form (ALIGN -> CLASSIFY, then the general kernel over
+// what ALIGN left over) or the general kernel alone; in the two-kernel form the narrow first tier with its second-tier launch,
+// the diagonal tier ahead of it and the diagonal tier's routing.
+static Plan plan_batch(const c2b_engine *e, const Batch &b, const Switches &sw)
+{
+    Plan plan;
+    WorkBlock *wb = (WorkBlock *)e->work.p;
     KParams P;
     memset(&P, 0, sizeof P);
-    P.reads = d_reads; P.offsets = d_offsets; P.n_reads = n_reads; P.count = d_count; P.qweight = d_qweight; P.ref_id = d_ref_id;
-    P.recs = d_recs; P.alns = d_alns; P.strings = d_strings; P.edits = d_edits;
-    P.W = (e->max_I + max_read_len + 31) & ~31; P.edit_cap = d_edits ? e->prm.edit_cap : 0;
+    P.reads = b.reads; P.offsets = b.offsets; P.n_reads = b.n_reads; P.count = b.count; P.qweight = b.qweight; P.ref_id = b.ref_id;
+    P.recs = b.recs; P.alns = b.alns; P.strings = b.strings; P.edits = b.edits;
+    P.W = (e->max_I + b.max_read_len + 31) & ~31; P.edit_cap = b.edits ? e->prm.edit_cap : 0;
     if (P.edit_cap == 0) P.edits = nullptr;
     P.refs = e->d_refs; P.n_refs = e->n_refs;
-    P.out_refs = d_ref_id ? 1 : e->n_refs; P.ops_refs = std::min(e->n_refs, (int)C2B_MAX_REFS);
+    P.out_refs = b.ref_id ? 1 : e->n_refs; P.ops_refs = std::min(e->n_refs, (int)C2B_MAX_REFS);
     P.go = e->prm.gap_open; P.ge = e->prm.gap_extend; P.seed_count = e->prm.seed_count; P.seed_min = e->prm.seed_min;
     P.flags = e->prm.flags; P.nq = e->prm.nq;
     memcpy(P.alpha, e->prm.alphabet, C2B_MAX_Q); memcpy(P.comp, e->prm.complement, C2B_MAX_Q);
     P.TS = e->scratch_TS;
-    auto at = [&](const DevBuf &b, size_t per_set) { return (char *)b.p + (size_t)set * per_set; };
-    P.tb = (uint32_t *)at(e->tb, e->set_tb); P.tb_words_per_warp = (int64_t)e->max_nrb * P.TS * 64;
-    P.tbb = getenv("C2B_NO_BAND") ? nullptr : (uint32_t *)at(e->tbb, e->set_tbb); P.tbb_words_per_warp = (int64_t)PK_BAND_SLOTS * 64;
-    P.tbq = getenv("C2B_NO_RING") ? nullptr : (uint32_t *)at(e->tbq, e->set_tbq);
-    P.bnd = (int32_t *)at(e->bnd, e->set_bnd); P.bnd_words_per_warp = 2 * 3 * (int64_t)P.TS;
-    P.opsbuf = (uint64_t *)at(e->ops, e->set_ops);
-    P.rgops = getenv("C2B_NO_MULTI_RING") ? nullptr : (uint64_t *)at(e->rgo, e->set_rgo);
-    P.stats = (unsigned long long *)e->work.p;
-    unsigned long long *wk = P.stats + 8 + 8 * set;       // [0] ALIGN / general hand-out counter, [1] widest alignment, [2] general kernel's counter after ALIGN, [3] left-over count
-    P.work_counter = wk; P.widest = wk + 1;
+    P.tb = (uint32_t *)e->tb.p; P.tb_words_per_warp = (int64_t)e->max_nrb * P.TS * 64;
+    P.tbb = (uint32_t *)e->tbb.p; P.tbb_words_per_warp = (int64_t)PK_BAND_SLOTS * 64;
+    P.tbq = (uint32_t *)e->tbq.p;
+    P.bnd = (int32_t *)e->bnd.p; P.bnd_words_per_warp = 2 * 3 * (int64_t)P.TS;
+    P.opsbuf = (uint64_t *)e->ops.p;
+    P.rgops = (uint64_t *)e->rgo.p;
+    P.wb = wb; P.work_counter = &wb->launch.align_next;
     P.vstride = e->vstride; P.hstride = e->hstride;
     P.forced_ops = e->forced_ops; P.forced_n = e->forced_n;
-    P.gops = d_gops; P.gmeta = d_gmeta; P.NW = P.W / 32;
+    P.gops = b.gops; P.gmeta = b.gmeta; P.NW = P.W / 32;
     P.pair_order = e->pair_order;
     P.lut = (const uint8_t *)e->lut.p;
-    P.stage_bytes = 0; P.stage_src = nullptr;
+    plan.one = e->n_refs == 1 || b.ref_id != nullptr;       // one candidate reference per read
     // two-kernel form: the configuration admits the ring-banded DP, op-stream buffers were supplied, nothing forces the
-    // general kernel (caller-supplied op streams, the A/B switches)
-    const bool split = e->split_ok && d_gops && d_gmeta && d_left && P.tbq && !e->forced_ops && !getenv("C2B_NO_SPLIT") &&
-                       (e->n_refs == 1 || d_ref_id != nullptr || (e->n_refs <= RG_MAX_REFS && e->split_all));
-    P.phase_sync = 0;
-    if (!split) {                                         // one-kernel form: warps of a phase set move in step (C2B_PHASE_WARPS: 0/1 = free-running, 2, 4, 8)
-        P.phase_sync = 4;
-        if (const char *v = getenv("C2B_PHASE_WARPS")) { const int k = atoi(v), a = k < 0 ? -k : k; P.phase_sync = (a == 2 || a == 4 || a == 8 || a == 16) ? k : 0; }
-        const int a = P.phase_sync < 0 ? -P.phase_sync : P.phase_sync;
-        const int nsets = a ? e->wpc / a : 0;
-        if (a > e->wpc || (a && e->wpc % a) || (P.phase_sync < 0 && (nsets & (nsets - 1)))) P.phase_sync = 0;
-        if (e->n_refs > 1 && !d_ref_id && getenv("C2B_NO_MULTI_PHASE")) P.phase_sync = 0;
-    }
-    const bool one = (e->n_refs == 1 || d_ref_id != nullptr) && !getenv("C2B_GENERIC_KERNEL");      // one candidate reference per read
-    RTCHK(rt_zero(wk, 64, cs));                           // this set's counters and widest alignment ([4], [5]: second-tier ALIGN launch)
-    if (d_gmeta) RTCHK(rt_zero(d_gmeta, (size_t)n_reads * P.out_refs * 4, cs));
-#ifndef C2B_EMU
+    // general kernel (caller-supplied op streams, C2B_NO_SPLIT)
+    const bool split = e->split_ok && b.gops && b.gmeta && b.left && !e->forced_ops && !sw.no_split &&
+                       (plan.one || (e->n_refs <= RG_MAX_REFS && e->split_all));
+    P.phase_sync = split ? 0 : 4;                         // one-kernel form: the warps of a phase set move in step
+    // reference 0's packed profile, staged into shared memory where it fits next to the kernel's per-warp state
     const RefDev &r0 = e->refdev[0];
-    const size_t tile = (size_t)e->prm.nq * e->prm.nq * r0.Ipad * 4;        // reference 0's packed profile
-    const bool can_stage = r0.pk_maxJ > 0 && !e->forced_ops && !getenv("C2B_NO_TMA_STAGE");
-    cudaEventRecord(e->ev0, cs);
+    const size_t tile = (size_t)e->prm.nq * e->prm.nq * r0.Ipad * 4;
+    const bool can_stage = r0.pk_maxJ > 0 && !e->forced_ops;
+    auto add = [&](StepKind kind, const KParams &K, int grid, int block, size_t smem) { plan.step[plan.n++] = Step{kind, K, grid, block, smem}; };
     if (split) {
         KParams A = P;
-        A.left = d_left; A.left_n = wk + 3;
-        A.discard_slab = getenv("C2B_NO_DISCARD") ? 0 : 1;
+        A.left = b.left;
         if (can_stage && tile <= (size_t)e->stage_cap_a) { A.stage_bytes = (int32_t)tile; A.stage_src = r0.prof2; }
-        const size_t smem_a = sizeof(ASmem) * e->wpc + 128 + (size_t)A.stage_bytes;
+        const size_t smem_a = sizeof(ASmem) * WARPS_PER_CTA + 128 + (size_t)A.stage_bytes;
         // narrow first tier (align_narrow16): reads in their given order (no pairing order = the caller's reads are of one
         // length, or unsorted -- then hardly any unit of sixteen qualifies), one candidate reference per read
-        const bool narrow = d_left2 && !P.pair_order && (e->n_refs == 1 || d_ref_id != nullptr) && !getenv("C2B_NO_NARROW");
-        if (narrow) { A.left2 = d_left2; A.left2_n = wk + 5; }
-        // diagonal tier ahead of the narrow one: reads it proves are done, the narrow tier works through the rest (wk[7] of them).
+        const bool narrow = b.left2 && !P.pair_order && plan.one && !sw.no_narrow;
+        if (narrow) A.left2 = b.left2;
+        // diagonal tier ahead of the narrow one: reads it proves are done, the narrow tier works through the rest.
         // A batch smaller than one narrow unit (16 reads) goes through the groups of eight anyway and keeps them whole.
-        const bool diag = narrow && d_left0 && e->diag_any && n_reads >= 16 && !getenv("C2B_NO_DIAG");
-        // routing: the diagonal tier puts the reads the narrow band cannot prove straight on the tier-2 list (wk[5]) and the
-        // rest on the narrow tier's list (wk[6]); CLASSIFY still takes all its unproved reads (wk[7])
-        const bool route = diag && d_left1 && !getenv("C2B_NO_ROUTE");
+        const bool diag = narrow && b.left0 && e->diag_any && b.n_reads >= 16 && !sw.no_diag;
+        // routing: the diagonal tier puts the reads the narrow band cannot prove straight on the tier-2 list and the rest on
+        // the narrow tier's list; CLASSIFY still takes all its unproved reads
+        const bool route = diag && b.left1 && !sw.no_route;
         if (diag) {
             KParams D = P;
-            D.left0 = d_left0; D.left0_n = wk + 7; D.diag_n = P.stats + 24;
-            if (route) { D.left1 = d_left1; D.left1_n = wk + 6; D.left2 = d_left2; D.left2_n = wk + 5; D.route = getenv("C2B_ROUTE_ALL") ? 2 : 1; }
-            const int64_t units = (n_reads + 31) / 32;
-            const int grid_d = (int)std::min<int64_t>((units + D_WARPS_PER_CTA - 1) / D_WARPS_PER_CTA, (int64_t)e->grid_a * 16);
-            c2b_diag_kernel<<<grid_d, D_WARPS_PER_CTA * 32, 0, cs>>>(D);
-            e->launches++;
-            A.pair_order = route ? d_left1 : d_left0; A.n_dev = route ? wk + 6 : wk + 7;
+            D.left0 = b.left0;
+            if (route) { D.left1 = b.left1; D.left2 = b.left2; D.route = sw.route_all ? 2 : 1; }
+            const int64_t units = (b.n_reads + 31) / 32;
+            add(STEP_DIAG, D, (int)std::min<int64_t>((units + D_WARPS_PER_CTA - 1) / D_WARPS_PER_CTA, (int64_t)e->grid_a * 16), D_WARPS_PER_CTA * 32, 0);
+            A.pair_order = route ? b.left1 : b.left0; A.n_dev = route ? &wb->launch.narrow_n : &wb->launch.diag_n;
         }
-        c2b_align_kernel<<<e->grid_a, e->wpc * 32, smem_a, cs>>>(A);
-        KParams B = P;                                        // CLASSIFY: every read in batch order, or the diagonal tier's list
-        B.pair_order = diag ? d_left0 : nullptr; B.n_dev = diag ? wk + 7 : nullptr;
+        add(STEP_ALIGN, A, e->grid_a, WARPS_PER_CTA * 32, smem_a);
         if (narrow) {                                         // second tier: what the narrow band did not settle, eight reads per group
             KParams A2 = A;
-            A2.left2 = nullptr; A2.left2_n = nullptr;
-            A2.pair_order = d_left2; A2.n_dev = wk + 5; A2.work_counter = wk + 4;
-            c2b_align_kernel<<<e->grid_a, e->wpc * 32, smem_a, cs>>>(A2);
-            e->launches++;
+            A2.left2 = nullptr;
+            A2.pair_order = b.left2; A2.n_dev = &wb->launch.tier2_n; A2.work_counter = &wb->launch.tier2_next;
+            add(STEP_ALIGN, A2, e->grid_a, WARPS_PER_CTA * 32, smem_a);
         }
-        if (one) c2b_classify_kernel<true><<<e->grid_b, B_WARPS_PER_CTA * 32, 0, cs>>>(B);
-        else c2b_classify_kernel<false><<<e->grid_b, B_WARPS_PER_CTA * 32, 0, cs>>>(B);
-        // the general kernel over ALIGN's left-over pairs (free-running warps, no ring-banded attempt)
-        P.pair_order = d_left; P.n_dev = wk + 3; P.work_counter = wk + 2; P.tbq = nullptr; P.rgops = nullptr;
-        P.tbb = nullptr;                                      // these pairs left the ring band: the banded slab would only cost a second DP
-        e->launches += 2;
+        KParams B = P;                                        // CLASSIFY: every read in batch order, or the diagonal tier's list
+        B.pair_order = diag ? b.left0 : nullptr; B.n_dev = diag ? &wb->launch.diag_n : nullptr;
+        add(STEP_CLASSIFY, B, e->grid_b, B_WARPS_PER_CTA * 32, 0);
+        // the general kernel over ALIGN's left-over pairs (free-running warps, no ring-banded attempt); these pairs left the
+        // ring band: the banded slab would only cost a second DP
+        P.pair_order = b.left; P.n_dev = &wb->launch.left_n; P.work_counter = &wb->launch.general_next;
+        P.tbq = nullptr; P.rgops = nullptr; P.tbb = nullptr;
     }
-    {
-        if (can_stage && tile <= (size_t)e->stage_cap) { P.stage_bytes = (int32_t)tile; P.stage_src = r0.prof2; }
-        const size_t smem = (sizeof(WarpSmem) + sizeof(QuadSmem)) * e->wpc + 128 + (size_t)P.stage_bytes;
-        if (one) c2b_align_classify_kernel<true><<<e->grid, e->wpc * 32, smem, cs>>>(P);
-        else c2b_align_classify_kernel<false><<<e->grid, e->wpc * 32, smem, cs>>>(P);
+    if (can_stage && tile <= (size_t)e->stage_cap) { P.stage_bytes = (int32_t)tile; P.stage_src = r0.prof2; }
+    add(STEP_GENERAL, P, e->grid, WARPS_PER_CTA * 32, (sizeof(WarpSmem) + sizeof(QuadSmem)) * WARPS_PER_CTA + 128 + (size_t)P.stage_bytes);
+    return plan;
+}
+
+#ifndef C2B_EMU
+static int run_plan(c2b_engine *e, const Plan &plan, rt_stream cs)
+{
+    cudaEventRecord(e->ev0, cs);
+    for (int k = 0; k < plan.n; k++) {
+        const Step &s = plan.step[k];
+        switch (s.kind) {
+        case STEP_DIAG: c2b_diag_kernel<<<s.grid, s.block, s.smem, cs>>>(s.P); break;
+        case STEP_ALIGN: c2b_align_kernel<<<s.grid, s.block, s.smem, cs>>>(s.P); break;
+        case STEP_CLASSIFY:
+            if (plan.one) c2b_classify_kernel<true><<<s.grid, s.block, s.smem, cs>>>(s.P);
+            else c2b_classify_kernel<false><<<s.grid, s.block, s.smem, cs>>>(s.P);
+            break;
+        case STEP_GENERAL:
+            if (plan.one) c2b_align_classify_kernel<true><<<s.grid, s.block, s.smem, cs>>>(s.P);
+            else c2b_align_classify_kernel<false><<<s.grid, s.block, s.smem, cs>>>(s.P);
+            break;
+        }
     }
     cudaEventRecord(e->ev1, cs);
     RTCHK(cudaGetLastError());
+    return C2B_OK;
+}
 #else
-    {
-        static WarpSmem S; static QuadSmem Q; static ASmem AS;
-        if (split) {
-            KParams A = P;
-            A.left = d_left; A.left_n = wk + 3;
-            emu::run_warp([&]() { asmem_init(A, AS); });
-            const bool narrow = d_left2 && !P.pair_order && (e->n_refs == 1 || d_ref_id != nullptr) && !getenv("C2B_NO_NARROW");
-            const int32_t *order = nullptr;                   // CLASSIFY's read order (nullptr: all reads)
-            int64_t n1 = n_reads;                             // reads CLASSIFY takes
-            if (narrow) {
-                A.left2 = d_left2; A.left2_n = wk + 5;
-                int64_t na = n_reads;                         // reads the narrow tier takes
-                if (d_left0 && e->diag_any && n_reads >= 16 && !getenv("C2B_NO_DIAG")) {    // diagonal tier, then the narrow tier over its list
-                    const bool route = d_left1 && !getenv("C2B_NO_ROUTE");
-                    KParams D = P;
-                    D.left0 = d_left0; D.left0_n = wk + 7; D.diag_n = P.stats + 24;
-                    if (route) { D.left1 = d_left1; D.left1_n = wk + 6; D.left2 = d_left2; D.left2_n = wk + 5; D.route = getenv("C2B_ROUTE_ALL") ? 2 : 1; }
-                    static DSmem DS;
-                    for (int64_t u = 0; 32 * u < n_reads; u++)
-                        emu::run_warp([&]() {
-                            dsmem_init(D, DS);
-                            ScAcc<1> acc; sc_init(acc);
-                            int kr = 0;
-                            const int k = diag_unit(D, DS, u, acc, kr), m = n_reads - 32 * u < 32 ? (int)(n_reads - 32 * u) : 32;
-                            sc_flush(acc, D);
-                            if (wp::lane() == 0) {
-                                wp::addg(D.diag_n, k); wp::addg(D.diag_n + 1, m - k);
-                                wp::addg(D.diag_n + 2, kr); wp::addg(D.diag_n + 3, kr); wp::addg(D.diag_n + 4, m - k - kr);
-                            }
-                        });
-                    A.pair_order = route ? d_left1 : d_left0; A.n_dev = route ? wk + 6 : wk + 7;
-                    na = (int64_t)*A.n_dev; n1 = (int64_t)wk[7]; order = d_left0;
-                }
-                for (int64_t w = 0; 16 * w < na; w++)
-                    emu::run_warp([&]() {
-                        if (!align_narrow16(A, AS, nullptr, w, 0)) {
-                            align_group(A, AS, nullptr, 2 * w, 0);
-                            wp::sync();
-                            if (8 * (2 * w + 1) < na) align_group(A, AS, nullptr, 2 * w + 1, 0);
-                        }
-                    });
-                KParams A2 = A;
-                A2.left2 = nullptr; A2.left2_n = nullptr; A2.pair_order = d_left2; A2.n_dev = wk + 5; A2.work_counter = wk + 4;
-                const int64_t n2 = (int64_t)*A2.n_dev;
-                for (int64_t w = 0; 8 * w < n2; w++) emu::run_warp([&]() { align_group(A2, AS, nullptr, w, 0); });
-            } else
-            for (int64_t w = 0; 8 * w < n_reads; w++) emu::run_warp([&]() { align_group(A, AS, nullptr, w, 0); });
-            static BSmem BS;
-            const int64_t total_bytes = d_offsets[n_reads];
-            for (int64_t x = 0; x < n1; x++) {
-                const int64_t rd = order ? order[x] : x;
-                if (one) emu::run_warp([&]() { ScAcc<1> acc; sc_init(acc); const BPreA a = classify_pre_a(P, rd); const BPre b = classify_pre_b<true>(P, rd, a, total_bytes);
-                                               if (b.go) { classify_stage<true>(b, BS); wp::sync(); classify_read<true>(P, rd, b, BS, acc); } sc_flush(acc, P); });
-                else emu::run_warp([&]() { ScAcc<RG_MAX_REFS> acc; sc_init(acc); const BPreA a = classify_pre_a(P, rd); const BPre b = classify_pre_b<false>(P, rd, a, total_bytes);
-                                            if (b.go) { classify_stage<false>(b, BS); wp::sync(); classify_read<false>(P, rd, b, BS, acc); } sc_flush(acc, P); });
-            }
-            P.pair_order = d_left; P.n_dev = wk + 3; P.work_counter = wk + 2; P.tbq = nullptr; P.rgops = nullptr; P.tbb = nullptr;
-        }
-        const int64_t nrd = P.n_dev ? (int64_t)*P.n_dev : n_reads;
-        if (P.n_dev) {                                      // left-over list: one pair per hand-out, like the kernel
-            for (int64_t w = 0; 2 * w < nrd; w++) {
-                if (one) emu::run_warp([&]() { process_item<true>(P, S, nullptr, w, 0); });
-                else emu::run_warp([&]() { process_item<false>(P, S, nullptr, w, 0); });
-            }
-        } else
-        for (int64_t w = 0; 8 * w < nrd; w++) {
-            wp::g_grp_syncs = 0;
-            if (one) emu::run_warp([&]() { process_group<true>(P, S, Q, nullptr, w, 0); });
-            else emu::run_warp([&]() { process_group<false>(P, S, Q, nullptr, w, 0); });
-            // every path through a work group must execute the same number of phase barriers (a mismatch deadlocks the GPU)
-            if (P.phase_sync && wp::g_grp_syncs != group_phases(P)) {
-                fprintf(stderr, "warp_emu: work group %lld executed %ld phase barriers, expected %d\n", (long long)w, wp::g_grp_syncs, group_phases(P));
-                abort();
-            }
+// The kernels' loops, each as a grid of one warp: the launch sequence's counters start at zero, so the warp's hand-outs walk
+// every item in order.
+static void run_phase_sets(const KParams &P, bool one, WarpSmem &S, QuadSmem &Q)
+{
+    // the general kernel's phase-set loop needs the warps of a set in step: here each group runs alone, and every path through
+    // a work group must execute the same number of phase barriers (a mismatch deadlocks the GPU)
+    for (int64_t w = 0; 8 * w < P.n_reads; w++) {
+        wp::g_grp_syncs = 0;
+        if (one) emu::run_warp([&]() { process_group<true>(P, S, Q, nullptr, w, 0); });
+        else emu::run_warp([&]() { process_group<false>(P, S, Q, nullptr, w, 0); });
+        if (P.phase_sync && wp::g_grp_syncs != group_phases(P)) {
+            fprintf(stderr, "warp_emu: work group %lld executed %ld phase barriers, expected %d\n", (long long)w, wp::g_grp_syncs, group_phases(P));
+            abort();
         }
     }
+}
+
+static int run_plan(c2b_engine *, const Plan &plan, rt_stream)
+{
+    static WarpSmem S; static QuadSmem Q; static ASmem AS; static BSmem BS; static DSmem DS;
+    for (int k = 0; k < plan.n; k++) {
+        const KParams &P = plan.step[k].P;
+        switch (plan.step[k].kind) {
+        case STEP_DIAG: emu::run_warp([&]() { diag_loop(P, DS, 0, 1); }); break;
+        case STEP_ALIGN: emu::run_warp([&]() { align_loop(P, AS, nullptr, 0); }); break;
+        case STEP_CLASSIFY:
+            if (plan.one) emu::run_warp([&]() { classify_loop<true>(P, BS, 0, 1); });
+            else emu::run_warp([&]() { classify_loop<false>(P, BS, 0, 1); });
+            break;
+        case STEP_GENERAL:
+            if (P.n_dev && plan.one) emu::run_warp([&]() { general_list_loop<true>(P, S, nullptr, 0); });
+            else if (P.n_dev) emu::run_warp([&]() { general_list_loop<false>(P, S, nullptr, 0); });
+            else run_phase_sets(P, plan.one, S, Q);
+            break;
+        }
+    }
+    return C2B_OK;
+}
 #endif
-    e->launches++;
+
+// One batch on compute stream `cs`: the launch sequence of plan_batch.
+static int launch_on(c2b_engine *e, rt_stream cs, Batch b)
+{
+    if (!e || !e->configured) return fail(e, C2B_E_STATE, "c2b_align_batch: engine not configured");
+    if (b.n_reads < 0 || !b.recs || !b.alns || (b.n_reads && (!b.reads || !b.offsets))) return fail(e, C2B_E_ARG, "c2b_align_batch: bad argument");
+    if (b.n_reads >= (1ll << 31)) return fail(e, C2B_E_LIMIT, "c2b_align_batch: more than 2^31 reads in one batch");
+    if (b.max_read_len < 1) b.max_read_len = 1;
+    if (b.max_read_len > C2B_MAX_READ_LEN) return fail(e, C2B_E_LIMIT, "c2b_align_batch: read longer than C2B_MAX_READ_LEN");
+    if ((int64_t)std::abs((long long)e->prm.gap_open) * b.max_read_len * e->max_I >= (1ll << 28))
+        return fail(e, C2B_E_LIMIT, "c2b_align_batch: gap_open * lengths exceeds the int32 score range");
+    if (int rc0 = score_range_ok(e, b.max_read_len, "c2b_align_batch")) return rc0;
+    if (!b.ref_id && e->n_refs > C2B_MAX_REFS)
+        return fail(e, C2B_E_LIMIT, "c2b_align_batch: more than C2B_MAX_REFS references need a per-read ref_id");
+    int rc = ensure_scratch(e, b.max_read_len);
+    if (rc) return rc;
+    if (b.n_reads == 0) return C2B_OK;
+    const Plan plan = plan_batch(e, b, read_switches());
+    RTCHK(rt_zero(&((WorkBlock *)e->work.p)->launch, sizeof(WorkBlock::Launch), cs));
+    if (b.gmeta) RTCHK(rt_zero(b.gmeta, (size_t)b.n_reads * (b.ref_id ? 1 : e->n_refs) * 4, cs));
+    if ((rc = run_plan(e, plan, cs))) return rc;
+    e->launches += plan.n;
     return C2B_OK;
 }
 
@@ -1170,9 +1003,9 @@ int c2b_align_batch_device(c2b_engine *e, const uint8_t *d_reads, const int64_t 
     const int W = (e->max_I + max_read_len + 31) & ~31, nr = d_ref_id ? 1 : e->n_refs;
     int rc = ensure_ops(e, e->gops, e->gmeta, e->left, e->left2, e->left0, e->left1, n_reads, nr, W);
     if (rc) return rc;
-    return launch_on(e, e->stream, 0, d_reads, d_offsets, n_reads, max_read_len, d_count, d_qweight, d_ref_id, d_recs,
+    return launch_on(e, e->stream, Batch{d_reads, d_offsets, n_reads, max_read_len, d_count, d_qweight, d_ref_id, d_recs,
                      d_alns, d_strings, d_edits, (uint64_t *)e->gops.p, (uint32_t *)e->gmeta.p, (int32_t *)e->left.p, (int32_t *)e->left2.p,
-                     (int32_t *)e->left0.p, (int32_t *)e->left1.p);
+                     (int32_t *)e->left0.p, (int32_t *)e->left1.p});
 }
 
 int c2b_ops_device(c2b_engine *e, void **d_ops, void **d_meta)
@@ -1219,40 +1052,40 @@ int64_t c2b_launch_count(const c2b_engine *e) { return e ? e->launches : 0; }
 int c2b_path_counts(c2b_engine *e, int64_t *pair_items, int64_t *single_items)
 {
     if (!e || !e->work.p) return fail(e, C2B_E_STATE, "c2b_path_counts: nothing launched yet");
-    int64_t v[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    RTCHK(rt_d2h(v, e->work.p, 64, e->stream));
+    WorkBlock v;
+    RTCHK(rt_d2h(&v, e->work.p, sizeof v, e->stream));
     RTCHK(rt_sync(e->stream));
-    // the ALIGN kernel counts reads ([5] kept by the ring, [6] sent on, [7] fully aligned); reported in pairs
-    e->band_reruns = v[4]; e->ring_pairs = (v[5] + 1) / 2; e->ring_fallbacks = (v[6] + 1) / 2;
+    // the ALIGN kernel counts reads (kept by the ring, sent on, fully aligned); reported in pairs
+    e->band_reruns = (int64_t)v.band_reruns; e->ring_pairs = (int64_t)(v.ring_kept + 1) / 2; e->ring_fallbacks = (int64_t)(v.ring_sent + 1) / 2;
     if (getenv("C2B_VERBOSE"))
         fprintf(stderr, "[c2b] counters: general kernel %lld pair items + %lld single items; ALIGN: %lld read x reference combinations kept "
-                        "by the ring, %lld sent to the full matrix, %lld reads settled\n", (long long)v[2], (long long)v[3], (long long)v[5],
-                (long long)v[6], (long long)v[7]);
-    if (pair_items) *pair_items = v[2] + (v[7] + 1) / 2;
-    if (single_items) *single_items = v[3];
+                        "by the ring, %lld sent to the full matrix, %lld reads settled\n", (long long)v.pair_items, (long long)v.single_items,
+                (long long)v.ring_kept, (long long)v.ring_sent, (long long)v.align_settled);
+    if (pair_items) *pair_items = (int64_t)(v.pair_items + (v.align_settled + 1) / 2);
+    if (single_items) *single_items = (int64_t)v.single_items;
     return C2B_OK;
 }
 
 int c2b_diag_counts(c2b_engine *e, int64_t *proved, int64_t *tier1, int64_t *tier2)
 {
     if (!e || !e->work.p) return fail(e, C2B_E_STATE, "c2b_diag_counts: nothing launched yet");
-    int64_t v[3] = {0, 0, 0};
-    RTCHK(rt_d2h(v, (unsigned long long *)e->work.p + 24, sizeof v, e->stream));
+    WorkBlock v;
+    RTCHK(rt_d2h(&v, e->work.p, sizeof v, e->stream));
     RTCHK(rt_sync(e->stream));
-    if (proved) *proved = v[0];
-    if (tier1) *tier1 = v[1];
-    if (tier2) *tier2 = v[2];
+    if (proved) *proved = (int64_t)v.diag_proved;
+    if (tier1) *tier1 = (int64_t)v.diag_listed;
+    if (tier2) *tier2 = (int64_t)v.tier2;
     return C2B_OK;
 }
 
 int c2b_route_counts(c2b_engine *e, int64_t *routed, int64_t *kept)
 {
     if (!e || !e->work.p) return fail(e, C2B_E_STATE, "c2b_route_counts: nothing launched yet");
-    int64_t v[2] = {0, 0};
-    RTCHK(rt_d2h(v, (unsigned long long *)e->work.p + 27, sizeof v, e->stream));
+    WorkBlock v;
+    RTCHK(rt_d2h(&v, e->work.p, sizeof v, e->stream));
     RTCHK(rt_sync(e->stream));
-    if (routed) *routed = v[0];
-    if (kept) *kept = v[1];
+    if (routed) *routed = (int64_t)v.routed;
+    if (kept) *kept = (int64_t)v.kept;
     return C2B_OK;
 }
 
@@ -1485,23 +1318,18 @@ static int align_batch_host(c2b_engine *e, const uint8_t *reads, const int64_t *
             e->pair_order = (const int32_t *)st.ord.p;
         }
         RTCHK(rt_record(st.in_done, e->s_in));
-        // C2B_TWO_STREAMS=1: consecutive chunks alternate between two compute streams (and the two scratch sets) so that the
-        // head of chunk c+1's ALIGN launch could fill the SMs the tails of chunk c's launches leave idle.  Measured slower
-        // end to end than one stream (two sets of ring slabs in flight, far more than the L2 holds) -- off.
-        const int set = (e->stream2 && getenv("C2B_TWO_STREAMS")) ? (ci & 1) : 0;
-        rt_stream cs = set ? e->stream2 : e->stream;
-        RTCHK(rt_wait(cs, st.in_done));
-        rc = launch_on(e, cs, set, (const uint8_t *)st.reads.p, (const int64_t *)st.off.p, n, (int32_t)maxJ,
+        RTCHK(rt_wait(e->stream, st.in_done));
+        rc = launch_on(e, e->stream, Batch{(const uint8_t *)st.reads.p, (const int64_t *)st.off.p, n, (int32_t)maxJ,
                        count ? (const int32_t *)st.cnt.p : nullptr, qweight ? (const int32_t *)st.qw.p : nullptr,
                        ref_id ? (const int32_t *)st.rid.p : nullptr, (c2b_read_rec *)st.recs.p,
                        (c2b_aln_rec *)st.alns.p, strings ? (uint8_t *)st.str.p : nullptr,
                        cap ? (c2b_edit *)st.ed.p : nullptr, (uint64_t *)st.gops.p, (uint32_t *)st.gmeta.p, (int32_t *)st.left.p, (int32_t *)st.left2.p, (int32_t *)st.left0.p,
-                       (int32_t *)st.left1.p);
+                       (int32_t *)st.left1.p});
         e->pair_order = nullptr;
         if (rc) return rc;
         // keep this batch's "widest alignment" before the next launch sequence resets it
-        RTCHK(cudaMemcpyAsyncOrCopy(st.maxlen.p, (const char *)e->work.p + (9 + 8 * set) * 8, 8, cs));
-        RTCHK(rt_record(st.k_done, cs));
+        RTCHK(cudaMemcpyAsyncOrCopy(st.maxlen.p, &((WorkBlock *)e->work.p)->launch.widest, 8, e->stream));
+        RTCHK(rt_record(st.k_done, e->stream));
         st.used = true;
         if (pend.any && (rc = flush(pend))) return rc;           // chunk ci-1: overlaps this chunk's kernels
         pend.any = true; pend.c0 = c0; pend.n = n; pend.set = ci & 1;
@@ -1509,7 +1337,6 @@ static int align_batch_host(c2b_engine *e, const uint8_t *reads, const int64_t *
     if (pend.any && (rc = flush(pend))) return rc;
     RTCHK(rt_sync(e->s_out));
     RTCHK(rt_sync(e->stream));
-    if (e->stream2) RTCHK(rt_sync(e->stream2));
     for (auto &st : e->stage) if ((rc = drain(st))) return rc;
     return C2B_OK;
 }

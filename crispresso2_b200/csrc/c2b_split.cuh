@@ -42,14 +42,14 @@ C2B_DEV int64_t read_at(const KParams &P, int64_t idx) { return P.pair_order ? (
 C2B_DEV void leftover_pair(const KParams &P, int64_t rdA, int64_t rdB)
 {
     if (wp::lane() == 0) {
-        const unsigned long long pos = wp::fetch_add(P.left_n, 2ull);
+        const unsigned long long pos = wp::fetch_add(&P.wb->launch.left_n, 2ull);
         P.left[pos] = (int32_t)rdA; P.left[pos + 1] = (int32_t)rdB;
     }
 }
 
 C2B_DEV void leftover_one(const KParams &P, int64_t rd)
 {
-    if (wp::lane() == 0) { const unsigned long long pos = wp::fetch_add(P.left_n, 1ull); P.left[pos] = (int32_t)rd; }
+    if (wp::lane() == 0) { const unsigned long long pos = wp::fetch_add(&P.wb->launch.left_n, 1ull); P.left[pos] = (int32_t)rd; }
 }
 
 // read -> alphabet codes for reads of at most RG_COMBO symbols; true if a symbol is outside the alphabet
@@ -425,7 +425,7 @@ C2B_DEV void align_group(const KParams &P, ASmem &S, const uint32_t *staged_prof
     }
 #ifndef C2B_EMU
     // the slab is dead now: drop its lines from L2 instead of writing them back to HBM (10 KB per read otherwise)
-    if (P.discard_slab && tbq && ringmask) {
+    if (tbq && ringmask) {
         const char *base = reinterpret_cast<const char *>(tbq);
         const int64_t bytes = (int64_t)P.TS * 64 * 4;
         for (int64_t o = (int64_t)lane * 128; o < bytes; o += 32 * 128)
@@ -433,9 +433,9 @@ C2B_DEV void align_group(const KParams &P, ASmem &S, const uint32_t *staged_prof
     }
 #endif
     if (lane == 0) {                                         // path statistics, in reads (the host reports pairs)
-        wp::addg(P.stats + 7, wp::popc(good2));
-        wp::addg(P.stats + 5, npass);
-        wp::addg(P.stats + 6, ntried - npass + nboth + 2 * (k1 - k0) * (4 - wp::popc(okmask)));
+        wp::addg(&P.wb->align_settled, wp::popc(good2));
+        wp::addg(&P.wb->ring_kept, npass);
+        wp::addg(&P.wb->ring_sent, ntried - npass + nboth + 2 * (k1 - k0) * (4 - wp::popc(okmask)));
     }
 #pragma unroll 1
     for (int q = 0; q < 4; q++) {
@@ -548,7 +548,7 @@ C2B_DEV bool align_narrow16(const KParams &P, ASmem &S, const uint32_t *staged_p
         }
     }
 #ifndef C2B_EMU
-    if (P.discard_slab) {                                    // the slab is dead now: drop its lines from L2
+    {                                                        // the slab is dead now: drop its lines from L2
         const char *base = reinterpret_cast<const char *>(tbq);
         const int64_t bytes = (int64_t)P.TS * 64 * 4;
         for (int64_t o = (int64_t)lane * 128; o < bytes; o += 32 * 128)
@@ -558,15 +558,74 @@ C2B_DEV bool align_narrow16(const KParams &P, ASmem &S, const uint32_t *staged_p
     // everything the narrow band did not settle: one entry each on the tier-2 list
     const uint32_t rest = 0xffffu & ~pass2;
     if (lane < 16 && ((rest >> lane) & 1u)) {
-        const unsigned long long pos = wp::fetch_add(P.left2_n, 1ull);
+        const unsigned long long pos = wp::fetch_add(&P.wb->launch.tier2_n, 1ull);
         P.left2[pos] = (int32_t)read_at(P, first + lane);
     }
     if (lane == 0) {
-        wp::addg(P.stats + 7, wp::popc(pass2));
-        wp::addg(P.stats + 5, wp::popc(pass2));
-        wp::addg(P.stats + 26, 16 - wp::popc(pass2));        // reads sent to the second tier (c2b_diag_counts)
+        wp::addg(&P.wb->align_settled, wp::popc(pass2));
+        wp::addg(&P.wb->ring_kept, wp::popc(pass2));
+        wp::addg(&P.wb->tier2, 16 - wp::popc(pass2));
     }
     return true;
+}
+
+// The ALIGN kernel's loop for warp `warp`: persistent, free-running warps pull work from a counter -- units of sixteen reads
+// with the narrow first tier (units it does not take run as two ordinary groups of eight), groups of eight without it.  The
+// work a warp is likely to get next has its bytes sent towards L2.  The number of warps is read from the grid where it is
+// used: passed in as a value it stays live across the DP calls, and the kernel spills more at its 128-register limit.
+C2B_DEV void align_loop(const KParams &P, ASmem &S, const uint32_t *staged_prof, int warp)
+{
+    const int lane = wp::lane();
+    asmem_init(P, S);
+    const int64_t nrd = nreads(P);
+    const unsigned ahead = (unsigned)wp::grid_warps();
+    if (P.left2) {
+        const unsigned total = (unsigned)((nrd + 15) / 16);
+        for (;;) {
+            unsigned w = 0;
+            if (lane == 0) w = (unsigned)wp::fetch_work(P.work_counter);
+            w = (unsigned)wp::shfl((int)w, 0);
+            if (w >= total) break;
+            if (w + ahead < total) {
+                const int64_t g = (int64_t)w + ahead;
+                if (!P.pair_order) {
+                    const int64_t last = 16 * g + 16 < nrd ? 16 * g + 16 : nrd;
+                    const int64_t a = P.offsets[16 * g] + (int64_t)lane * 128;
+                    if (a < P.offsets[last]) wp::prefetch_l2(P.reads + a);
+                } else {                                        // reads of the diagonal tier's list: two lanes per read
+                    const int64_t x = 16 * g + (lane >> 1);
+                    if (x < nrd) {
+                        const int64_t rd = read_at(P, x);
+                        const int64_t b1 = P.offsets[rd + 1];
+                        for (int64_t a = (P.offsets[rd] & ~(int64_t)127) + (int64_t)(lane & 1) * 128; a < b1; a += 256)
+                            wp::prefetch_l2(P.reads + a);
+                    }
+                }
+            }
+            if (!align_narrow16(P, S, staged_prof, (int64_t)w, warp)) {
+                align_group(P, S, staged_prof, 2 * (int64_t)w, warp);
+                wp::sync();
+                if (8 * (2 * (int64_t)w + 1) < nrd) align_group(P, S, staged_prof, 2 * (int64_t)w + 1, warp);
+            }
+            wp::sync();
+        }
+        return;
+    }
+    const unsigned total = (unsigned)((nrd + 7) / 8);
+    for (;;) {
+        unsigned w = 0;
+        if (lane == 0) w = (unsigned)wp::fetch_work(P.work_counter);
+        w = (unsigned)wp::shfl((int)w, 0);
+        if (w >= total) break;
+        if (w + ahead < total && !P.pair_order) {
+            const int64_t g = (int64_t)w + ahead;
+            const int64_t last = 8 * g + 8 < nrd ? 8 * g + 8 : nrd;
+            const int64_t a = P.offsets[8 * g] + (int64_t)lane * 128;
+            if (a < P.offsets[last]) wp::prefetch_l2(P.reads + a);
+        }
+        align_group(P, S, staged_prof, (int64_t)w, warp);
+        wp::sync();
+    }
 }
 
 // ------------------------------------------------------------------------------------------------- CLASSIFY
@@ -619,7 +678,7 @@ C2B_DEV void sc_flush(ScAcc<NA> &A, const KParams &P)
         if (A.ref[x] >= 0 && A.v[x] != 0 && lane < C2B_NSCAL) wp::addg(P.refs[A.ref[x]].scal + lane, A.v[x]);
         A.v[x] = 0; A.ref[x] = -1;
     }
-    if (lane == 0 && A.wmax) wp::maxg(P.widest, (unsigned long long)A.wmax);      // widest alignment of the launch
+    if (lane == 0 && A.wmax) wp::maxg(&P.wb->launch.widest, (unsigned long long)A.wmax);      // widest alignment of the launch
     A.wmax = 0;
 }
 
@@ -1107,6 +1166,44 @@ C2B_DEV void classify_read(const KParams &P, int64_t rd, const BPre &pre, const 
     if (lane == 0) P.recs[rd] = rec;
 }
 
+// The CLASSIFY kernel's loop for warp `warp` of `nwarps`: one aligned read per warp, reads strided over the warps -- every
+// read, or (after the diagonal tier, which classifies the reads it proves) the entries of its list: P.pair_order, *P.n_dev.
+template <bool ONE>
+C2B_DEV void classify_loop(const KParams &P, BSmem &S, int64_t warp, int64_t nwarps)
+{
+    const int64_t nw = nwarps;
+    const int64_t total_bytes = P.offsets[P.n_reads];
+    const int64_t n = nreads(P);
+    int64_t x = warp;                                                    // position in the read order
+    if (x >= n) return;
+    ScAcc<ONE ? 1 : RG_MAX_REFS> acc;
+    sc_init(acc);
+    // two-deep input pipeline: stage A of position x + 2 nw and stage B of x + nw are in flight while x is classified; the
+    // read at x + 3 nw is looked up one iteration before its stage A needs it (a list entry, then its offsets: two round trips)
+    int32_t rd = (int32_t)read_at(P, x), rd1 = 0, rd2 = 0;
+    BPreA a1 = classify_pre_a(P, rd);
+    BPre pre = classify_pre_b<ONE>(P, rd, a1, total_bytes);
+    if (x + nw < n) { rd1 = (int32_t)read_at(P, x + nw); a1 = classify_pre_a(P, rd1); }
+    if (x + 2 * nw < n) rd2 = (int32_t)read_at(P, x + 2 * nw);
+    while (x < n) {
+        const BPre cur = pre;
+        const int32_t rc = rd;
+        if (cur.go) classify_stage<ONE>(cur, S);
+        wp::sync();
+        const int64_t nxt = x + nw;
+        if (nxt < n) {
+            pre = classify_pre_b<ONE>(P, rd1, a1, total_bytes);
+            rd = rd1;
+            if (nxt + nw < n) { a1 = classify_pre_a(P, rd2); rd1 = rd2; }
+            if (nxt + 2 * nw < n) rd2 = (int32_t)read_at(P, nxt + 2 * nw);
+        }
+        if (cur.go) classify_read<ONE>(P, rc, cur, S, acc);
+        wp::sync();
+        x = nxt;
+    }
+    sc_flush(acc, P);
+}
+
 // ---------------------------------------------------------------------------------------- diagonal tier (tier 0)
 // A read as long as its amplicon whose ungapped score on the main diagonal beats every other path is aligned there, with no
 // DP: it scores strictly above RefDev::dg_thr4 (the bound on paths with an interior gap run, on offset diagonals past dg_S and
@@ -1387,13 +1484,38 @@ C2B_DEV int diag_unit(const KParams &P, DSmem &S, int64_t u, ScAcc<1> &A, int &r
         if (v == DG_ROUTE) route |= 1u << x;
         wp::sync();
     }
-    list_append(P.left0, P.left0_n, fail, first);   // every unproved read: CLASSIFY's list
+    list_append(P.left0, &P.wb->launch.diag_n, fail, first);   // every unproved read: CLASSIFY's list
     if (P.route) {                                   // routing: the narrow tier's list and the tier-2 list
-        list_append(P.left1, P.left1_n, fail & ~route, first);
-        list_append(P.left2, P.left2_n, route, first);
+        list_append(P.left1, &P.wb->launch.narrow_n, fail & ~route, first);
+        list_append(P.left2, &P.wb->launch.tier2_n, route, first);
     }
     routed = wp::popc(route);
     return n - wp::popc(fail);
+}
+
+// The diagonal tier's loop for warp `warp` of `nwarps`: units of 32 consecutive reads strided over the warps; the warp's
+// counts go to the work block once, at the end
+C2B_DEV void diag_loop(const KParams &P, DSmem &S, int64_t warp, int64_t nwarps)
+{
+    dsmem_init(P, S);
+    ScAcc<1> acc;
+    sc_init(acc);
+    const int64_t units = (P.n_reads + 31) / 32;
+    int proved = 0, seen = 0, routed = 0;
+    for (int64_t u = warp; u < units; u += nwarps) {
+        int k = 0;
+        proved += diag_unit(P, S, u, acc, k);
+        routed += k;
+        seen += P.n_reads - 32 * u < 32 ? (int)(P.n_reads - 32 * u) : 32;
+        wp::sync();
+    }
+    sc_flush(acc, P);
+    if (wp::lane() == 0 && seen) {
+        WorkBlock &wb = *P.wb;
+        wp::addg(&wb.diag_proved, proved); wp::addg(&wb.diag_listed, seen - proved);
+        wp::addg(&wb.tier2, routed);                    // tier-2 reads: routed here, and the narrow tier's failures
+        wp::addg(&wb.routed, routed); wp::addg(&wb.kept, seen - proved - routed);
+    }
 }
 
 }  // namespace c2b

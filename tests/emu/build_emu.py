@@ -5,7 +5,8 @@ import subprocess
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 SO = os.path.join(HERE, "libc2b200_emu.so")
-SRC = [os.path.join(ROOT, "crispresso2_b200", "csrc", f) for f in ("c2b_engine.cu", "c2b_core.cuh", "c2b_fastq.cpp", "c2b_split.cuh", "c2b_alleles.cpp", "c2b_fastq_int.h", "c2b_paired.cpp")] + \
+SRC = [os.path.join(ROOT, "crispresso2_b200", "csrc", f) for f in ("c2b_engine.cu", "c2b_core.cuh", "c2b_fastq.cpp", "c2b_split.cuh", "c2b_alleles.cpp", "c2b_fastq_int.h", "c2b_paired.cpp",
+                                                                     "c2b_annotate.cuh")] + \
       [os.path.join(HERE, "warp_emu.h"), os.path.join(ROOT, "include", "c2b200.h")]
 
 
