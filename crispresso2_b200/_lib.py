@@ -80,7 +80,7 @@ assert ALN_DTYPE.itemsize == 32 and REC_DTYPE.itemsize == 16 and EDIT_DTYPE.item
 
 EXPORTS = ["c2b_create", "c2b_destroy", "c2b_last_error", "c2b_configure", "c2b_set_edit_cap", "c2b_string_width", "c2b_align_batch",
            "c2b_align_batch_compact", "c2b_ops_words", "c2b_expand_alignment", "c2b_expand_batch", "c2b_ops_device",
-           "c2b_align_batch_device", "c2b_set_pair_order", "c2b_sync", "c2b_stream", "c2b_last_kernel_ms", "c2b_launch_count", "c2b_path_counts", "c2b_band_reruns", "c2b_ring_counts", "c2b_diag_counts", "c2b_route_counts",
+           "c2b_align_batch_device", "c2b_set_pair_order", "c2b_sync", "c2b_stream", "c2b_last_kernel_ms", "c2b_launch_count", "c2b_path_counts", "c2b_band_reruns", "c2b_ring_counts", "c2b_diag_counts", "c2b_route_counts", "c2b_diag_popcount_reads",
            "c2b_counts_layout", "c2b_counts_hist_layout", "c2b_counts_reset", "c2b_counts_read", "c2b_counts_device", "c2b_global_align",
            "c2b_classify_aligned", "c2b_classify_aligned_flags", "c2b_host_alloc", "c2b_host_free",
            "c2b_fastq_dedup", "c2b_fastq_dedup_buffer", "c2b_fastq_gpu_available", "c2b_fastq_dedup_gpu", "c2b_fastq_dedup_gpu_buffer", "c2b_sam_dedup_gpu_buffer", "c2b_sam_dedup_buffer", "c2b_fastq_n_reads", "c2b_fastq_n_unique", "c2b_fastq_max_len",
@@ -157,6 +157,8 @@ def load(path=None):
     L.c2b_diag_counts.argtypes = [vp, C.POINTER(i64), C.POINTER(i64), C.POINTER(i64)]
     L.c2b_route_counts.restype = C.c_int
     L.c2b_route_counts.argtypes = [vp, C.POINTER(i64), C.POINTER(i64)]
+    L.c2b_diag_popcount_reads.restype = C.c_int
+    L.c2b_diag_popcount_reads.argtypes = [vp, C.POINTER(i64)]
     L.c2b_counts_layout.restype = C.c_int
     L.c2b_counts_layout.argtypes = [vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), C.POINTER(i32)]
     L.c2b_counts_hist_layout.restype = C.c_int

@@ -62,6 +62,10 @@ C2B_DEV int grid_warps() { return (int)(gridDim.x * (blockDim.x >> 5)); }
 // shared-state-space accesses through a 32-bit address kept in a register (no generic-address arithmetic in hot loops)
 C2B_DEV uint32_t smem_addr(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 C2B_DEV uint32_t lds_u8(uint32_t a) { uint32_t v; asm volatile("ld.shared.u8 %0, [%1];" : "=r"(v) : "r"(a)); return v; }
+// 16 bytes global -> shared that land in the background (cp.async); wait_async: every copy this thread issued has landed
+C2B_DEV void cp_async16(void *dst, const void *src)
+{ asm volatile("cp.async.ca.shared.global [%0], [%1], 16;" ::"r"(smem_addr(dst)), "l"(__cvta_generic_to_global(src)) : "memory"); }
+C2B_DEV void wait_async() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 C2B_DEV uint4 lds_v4(uint32_t a) { uint4 v; asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(a)); return v; }
 C2B_DEV uint2 ldcg2(const uint2 *p) { return __ldcg(p); }
 C2B_DEV uint32_t funnel_r(uint32_t lo, uint32_t hi, int sh) { return __funnelshift_r(lo, hi, sh); }   // (hi:lo) >> sh
@@ -90,6 +94,8 @@ C2B_DEV unsigned long long fetch_add(unsigned long long *p, unsigned long long v
 #include "warp_emu.h"   // provides C2B_DEV, C2B_DEVNOINL, int4/uint4 and namespace wp
 namespace wp {
 C2B_DEV int grid_warps() { return 1; }                  // the emulator runs a kernel's loop as a grid of one warp
+C2B_DEV void cp_async16(void *dst, const void *src) { memcpy(dst, src, 16); }
+C2B_DEV void wait_async() {}
 }  // namespace wp
 #endif
 
@@ -131,6 +137,9 @@ struct RefDev {
     // edge-run scores of the offsets 1..dg_S on either side is aligned on the main diagonal, no DP needed
     int32_t dg_ok, dg_S, dg_thr4;
     int32_t dg_c4[2 * 4 + 1];      // [s + 4]: 4 x (gap costs + incentives) of the path on offset diagonal s (edge runs only)
+    // every amplicon base has a code in 0..3 and the scores it meets from codes 0..3 are two-valued: dg_a4 = 4 x the score of
+    // the amplicon's own code, dg_b4 = 4 x that of any other; the tier then scores a read of codes 0..3 by popcounts
+    int32_t dg_two, dg_a4, dg_b4;
     // routing of the tier's unproved reads (route_read, DESIGN.md section 3): a read whose lower bound on its best one-gap
     // path does not beat rt_thr (the narrow band's ring_bound at J == I) goes straight to the wide ring
     int32_t rt_ok, rt_thr;
@@ -152,6 +161,7 @@ struct WorkBlock {
     // cumulative, the diagonal tier (c2b_diag_counts, c2b_route_counts): reads proved, put on its list, sent to the second tier
     // (routed there or failed by the narrow tier), routed, kept for the narrow tier
     unsigned long long diag_proved, diag_listed, tier2, routed, kept;
+    unsigned long long diag_popc;          // cumulative (c2b_diag_popcount_reads): reads the diagonal tier scored by popcounts
     struct Launch {                        // zeroed at the start of every launch sequence
         // work hand-out counters: ALIGN (or the general kernel alone), the second-tier ALIGN launch, the general kernel after ALIGN
         unsigned long long align_next, tier2_next, general_next;

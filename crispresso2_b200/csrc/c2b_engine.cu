@@ -638,6 +638,21 @@ int c2b_configure(c2b_engine *e, const c2b_params *p, int32_t n_refs, const c2b_
                 d.dg_c4[s + 4] = (int32_t)(4 * (s == 0 ? 0 : 2 * ge * t + gi0 + (s > 0 ? rf.gap_incentive[I - std::min<int64_t>(t, I)] : t * gI)));
             }
             if (!d.dg_ok) { d.dg_S = 0; d.dg_thr4 = 0; }
+            // two-valued scores over codes 0..3 (EDNAFULL over ACGT: 5 / -4): the tier's sums become match counts
+            const int nq4 = std::min(p->nq, 4);
+            int64_t a = 0, b = 0;
+            bool two = d.dg_ok && I <= 256, have_b = false;
+            for (int i = 0; i < I && two; i++) {
+                if (rcode[i] >= nq4) { two = false; break; }
+                for (int q = 0; q < nq4; q++) {
+                    const int64_t v = rf.score_rows[(size_t)q * I + i];
+                    if (q == rcode[i]) { if (i == 0) a = v; else if (v != a) two = false; }
+                    else if (!have_b) { b = v; have_b = true; }
+                    else if (v != b) two = false;
+                }
+            }
+            two = two && 4 * (std::abs(a) + std::abs(b)) * I < (1ll << 30);      // the grouped sums stay inside int32
+            d.dg_two = two; d.dg_a4 = two ? (int32_t)(4 * a) : 0; d.dg_b4 = two ? (int32_t)(4 * b) : 0;
         }
         {   // routing of the diagonal tier's unproved reads (route_read, DESIGN.md section 3)
             const int nq4 = std::min(p->nq, 4);
@@ -1075,6 +1090,16 @@ int c2b_diag_counts(c2b_engine *e, int64_t *proved, int64_t *tier1, int64_t *tie
     if (proved) *proved = (int64_t)v.diag_proved;
     if (tier1) *tier1 = (int64_t)v.diag_listed;
     if (tier2) *tier2 = (int64_t)v.tier2;
+    return C2B_OK;
+}
+
+int c2b_diag_popcount_reads(c2b_engine *e, int64_t *reads)
+{
+    if (!e || !e->work.p) return fail(e, C2B_E_STATE, "c2b_diag_popcount_reads: nothing launched yet");
+    WorkBlock v;
+    RTCHK(rt_d2h(&v, e->work.p, sizeof v, e->stream));
+    RTCHK(rt_sync(e->stream));
+    if (reads) *reads = (int64_t)v.diag_popc;
     return C2B_OK;
 }
 

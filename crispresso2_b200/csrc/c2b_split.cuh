@@ -52,15 +52,15 @@ C2B_DEV void leftover_one(const KParams &P, int64_t rd)
     if (wp::lane() == 0) { const unsigned long long pos = wp::fetch_add(&P.wb->launch.left_n, 1ull); P.left[pos] = (int32_t)rd; }
 }
 
-// read -> alphabet codes for reads of at most RG_COMBO symbols; true if a symbol is outside the alphabet
-C2B_DEV bool load_codes_a(const KParams &P, const uint8_t *lut, int64_t off, int J, uint8_t *fw, uint8_t *rc)
+// read (its J bytes at src) -> alphabet codes for reads of at most RG_COMBO symbols; true if a symbol is outside the alphabet
+C2B_DEV bool load_codes_a(const KParams &P, const uint8_t *lut, const uint8_t *src, int J, uint8_t *fw, uint8_t *rc)
 {
     const int lane = wp::lane();
     bool bad = false;
     for (int base = 0; base < J; base += 128) {
         uint8_t ch[4];
 #pragma unroll
-        for (int e = 0; e < 4; e++) { const int p = base + lane + 32 * e; ch[e] = p < J ? P.reads[off + p] : (uint8_t)P.alpha[0]; }
+        for (int e = 0; e < 4; e++) { const int p = base + lane + 32 * e; ch[e] = p < J ? src[p] : (uint8_t)P.alpha[0]; }
 #pragma unroll
         for (int e = 0; e < 4; e++) {
             const int p = base + lane + 32 * e;
@@ -259,7 +259,7 @@ C2B_DEV void align_group(const KParams &P, ASmem &S, const uint32_t *staged_prof
         const int J = (int)(P.offsets[rdA + 1] - P.offsets[rdA]);
         bool bad = false;
 #pragma unroll 1
-        for (int x = 0; x < 2; x++) bad |= load_codes_a(P, S.lut, P.offsets[x ? rdB : rdA], J, S.fw[x], S.rc[x]);
+        for (int x = 0; x < 2; x++) bad |= load_codes_a(P, S.lut, P.reads + P.offsets[x ? rdB : rdA], J, S.fw[x], S.rc[x]);
         wp::sync();
         int mAB = 0; bool agree = true;
         uint32_t bothq[RG_MAX_REFS] = {0, 0, 0, 0};
@@ -382,7 +382,7 @@ C2B_DEV void align_group(const KParams &P, ASmem &S, const uint32_t *staged_prof
                 wp::sync();
                 if (kind) {
                     const int64_t rdx = read_at(P, 2 * (first + q) + (kind - 1));
-                    load_codes_a(P, S.lut, P.offsets[rdx], Jp, S.fw[0], S.rc[0]);
+                    load_codes_a(P, S.lut, P.reads + P.offsets[rdx], Jp, S.fw[0], S.rc[0]);
                     wp::sync();
                     for (int p = lane; p < Jp; p += 32) S.fw[1][p] = (uint8_t)(S.fw[0][p] * P.nq + S.rc[0][p]);
                     combo = S.fw[1];
@@ -485,8 +485,8 @@ C2B_DEV bool align_narrow16(const KParams &P, ASmem &S, const uint32_t *staged_p
 #pragma unroll 1
     for (int q = 0; q < 8; q++) {
         const int64_t rdA = read_at(P, first + 2 * q), rdB = read_at(P, first + 2 * q + 1);
-        bool badA = load_codes_a(P, S.lut, P.offsets[rdA], J, S.fw[0], S.rc[0]);
-        bool badB = load_codes_a(P, S.lut, P.offsets[rdB], J, S.fw[1], S.rc[1]);
+        bool badA = load_codes_a(P, S.lut, P.reads + P.offsets[rdA], J, S.fw[0], S.rc[0]);
+        bool badB = load_codes_a(P, S.lut, P.reads + P.offsets[rdB], J, S.fw[1], S.rc[1]);
         wp::sync();
         int m = 0;
 #pragma unroll 1
@@ -1215,19 +1215,32 @@ C2B_DEV void classify_loop(const KParams &P, BSmem &S, int64_t warp, int64_t nwa
 // (P.left1) or straight onto the tier-2 list (P.left2) that the wide ring works through (route_read).
 constexpr int DG_PROVED = 0, DG_KEEP = 1, DG_ROUTE = 2;     // diag_read: proved / for the narrow tier / for the wide ring
 struct DSmem {                                         // diagonal tier, per warp
-    uint4 pl[2][10];                                   // route_read: the read's and the reference's codes as bit planes, 32 columns per word
+    uint4 pl[2][10];                                   // the read's and the reference's codes as bit planes, 32 columns per word
+    uint8_t raw[2][RG_COMBO + 32];                     // the bytes of the unit's next reads, from the 16-byte line at or below each (diag_stage)
     int32_t pl_ref;                                    // reference whose planes are in pl[1] (-1: none)
     uint8_t fw[RG_COMBO], rc[RG_COMBO];
     uint8_t lut[256];
     int64_t off[33];
+    int64_t total_bytes;                               // of the read buffer
     int32_t ref[32], cnt[32], qw[32];
+    int32_t npop;                                      // reads this warp scored by popcounts
 };
+
+// Bit planes of alphabet codes, 32 columns per word (x: code bit 0, y: code bit 1, z: code in 0..3): the columns where two
+// words hold the same code in 0..3; columns x + t of the word pair (lo, hi), 0 <= t < 32; the columns below n of a word
+C2B_DEV uint32_t pl_match(uint4 a, uint4 b) { return ~((a.x ^ b.x) | (a.y ^ b.y)) & a.z & b.z; }
+C2B_DEV uint4 pl_shifted(uint4 lo, uint4 hi, int t)
+{
+    return make_uint4(wp::funnel_r(lo.x, hi.x, t), wp::funnel_r(lo.y, hi.y, t), wp::funnel_r(lo.z, hi.z, t), 0u);
+}
+C2B_DEV uint32_t pl_below(int n) { return n >= 32 ? ~0u : n <= 0 ? 0u : (1u << n) - 1u; }
 
 // classify_read<true> for a read the tier proved: I columns of OP_M on the main diagonal, no gap column.  c: the read as
 // alphabet codes in the aligned strand; column p's read character is P.alpha[c[p]], which is how col_decode spells it (the
-// lookup table maps exactly the alphabet's characters, and a read with any other symbol is never proved).
+// lookup table maps exactly the alphabet's characters, and a read with any other symbol is never proved).  planes: the read
+// and the amplicon hold codes 0..3 only and S.pl holds their bit planes (diag_read), so a column differs iff its codes do.
 C2B_DEV void diag_classify(const KParams &P, const DSmem &S, const RefDev &R, const uint8_t *c, int64_t rd, int r, int strand,
-                           long long cnt, long long w, ScAcc<1> &A)
+                           long long cnt, long long w, ScAcc<1> &A, bool planes)
 {
     const int lane = wp::lane(), I = R.I;
     const uint32_t lt = (1u << lane) - 1u;
@@ -1238,16 +1251,31 @@ C2B_DEV void diag_classify(const KParams &P, const DSmem &S, const RefDev &R, co
     uint8_t *o_read = P.strings ? P.strings + (slot * 2) * (int64_t)P.W + P.W - I : nullptr;
     int match = 0;
     uint32_t irr = 0, mmis = 0;
+    if (planes) {                                    // the ballots from the planes; the strings' loads overlap
+        mmis = lane < nsteps ? ~pl_match(S.pl[0][lane], S.pl[1][lane]) & pl_below(I - 32 * lane) : 0u;
+        int k = wp::popc(mmis);
+#pragma unroll
+        for (int d = 16; d >= 1; d >>= 1) k += wp::shfl_xor(k, d);
+        match = I - k;
+        irr = (wp::shflu(mmis, 0) & 1u) | ((wp::shflu(mmis, nsteps - 1) >> ((I - 1) & 31)) & 1u);
+        if (o_read)
+#pragma unroll 4
+            for (int m = 0; m < nsteps; m++) {
+                const int p = 32 * m + lane;
+                if (p < I) { o_read[p] = (uint8_t)P.alpha[c[p]]; o_read[P.W + p] = R.asc[p]; }
+            }
+    } else {
 #pragma unroll 1
-    for (int m = 0; m < nsteps; m++) {
-        const int p = 32 * m + lane;
-        const bool valid = p < I;
-        const uint32_t rdc = valid ? P.alpha[c[p]] : 0u, rfc = valid ? R.asc[p] : 0u;
-        const uint32_t Bmis = wp::ballot(valid && rdc != rfc);
-        match += wp::popc(wp::ballot(valid && rdc == rfc));
-        irr |= wp::ballot(valid && (p == 0 || p == I - 1) && rdc != rfc);
-        if (o_read && valid) { o_read[p] = (uint8_t)rdc; o_read[P.W + p] = (uint8_t)rfc; }
-        if (lane == m) mmis = Bmis;
+        for (int m = 0; m < nsteps; m++) {
+            const int p = 32 * m + lane;
+            const bool valid = p < I;
+            const uint32_t rdc = valid ? P.alpha[c[p]] : 0u, rfc = valid ? R.asc[p] : 0u;
+            const uint32_t Bmis = wp::ballot(valid && rdc != rfc);
+            match += wp::popc(wp::ballot(valid && rdc == rfc));
+            irr |= wp::ballot(valid && (p == 0 || p == I - 1) && rdc != rfc);
+            if (o_read && valid) { o_read[p] = (uint8_t)rdc; o_read[P.W + p] = (uint8_t)rfc; }
+            if (lane == m) mmis = Bmis;
+        }
     }
     ColOut co; co.n_match = match; co.irregular = irr != 0;
     c2b_read_rec rec; rec.winner_mask = 0; rec.best_score_milli = -1000; rec.best_ref = -1; rec.n_winners = 0;
@@ -1316,36 +1344,18 @@ C2B_DEV void diag_classify(const KParams &P, const DSmem &S, const RefDev &R, co
 // at least the least score).  Lane s + 16 takes offset s and finds its best split among the block ends p = 32, 64, ..
 // (clamped to I - t); the best lane's 64 splits around its block end are then scanned exactly, incentives included.  A read
 // is kept iff that lower bound beats rt_thr; any other read costs the wide ring what the narrow tier would have wasted on it.
-C2B_DEV int route_read(const KParams &P, DSmem &S, const RefDev &R, int r, const uint8_t *c, int D)
+// S.pl holds the read's and the amplicon's bit planes (diag_read).
+C2B_DEV int route_read(const RefDev &R, const DSmem &S, int D)
 {
     if (!R.rt_ok || D > R.rt_thr) return DG_KEEP;            // no bound for this reference / the diagonal alone beats it
     const int lane = wp::lane(), I = R.I, nb = (I + 31) >> 5;
-    auto match = [](uint4 a, uint4 b) { return ~((a.x ^ b.x) | (a.y ^ b.y)) & a.z & b.z; };
-    auto shifted = [](uint4 lo, uint4 hi, int t) {           // columns x + t of the word pair (lo, hi), 0 <= t < 32
-        return make_uint4(wp::funnel_r(lo.x, hi.x, t), wp::funnel_r(lo.y, hi.y, t), wp::funnel_r(lo.z, hi.z, t), 0u);
-    };
-    auto below = [](int n) -> uint32_t { return n >= 32 ? ~0u : n <= 0 ? 0u : (1u << n) - 1u; };
-    // bit planes of the read (aligned strand) and, once per reference, of the amplicon; words nb and nb + 1 are zero
-    for (int b = 0; b < nb; b++) {
-        const int x = 32 * b + lane, q = x < I ? c[x] : 255;
-        const uint32_t p0 = wp::ballot(q & 1), p1 = wp::ballot(q & 2), v = wp::ballot(q < 4);
-        if (lane == 0) S.pl[0][b] = make_uint4(p0, p1, v, 0u);
-    }
-    if (lane < 2) S.pl[0][nb + lane] = make_uint4(0u, 0u, 0u, 0u);
-    const bool fresh = S.pl_ref != r;
-    wp::sync();
-    if (fresh) {
-        if (lane < nb + 2) S.pl[1][lane] = R.rt_pl[lane];
-        if (lane == 0) S.pl_ref = r;
-    }
-    wp::sync();
     const int s = lane - 16, t = s < 0 ? -s : s, cs = R.rt_c[lane];
     const uint4 *Ap = S.pl[s < 0 ? 0 : 1], *Bp = S.pl[s < 0 ? 1 : 0];
     int run = 0, best = RT_OFF, bb = 1, mst = 0;             // run: F(32 (b + 1)) - mst; bb: first block end attaining best
 #pragma unroll 1
     for (int b = 0; b < nb; b++) {
-        const uint32_t m0 = match(S.pl[0][b], S.pl[1][b]) & below(I - t - 32 * b);
-        const uint32_t ms = match(Ap[b], shifted(Bp[b], Bp[b + 1], t));
+        const uint32_t m0 = pl_match(S.pl[0][b], S.pl[1][b]) & pl_below(I - t - 32 * b);
+        const uint32_t ms = pl_match(Ap[b], pl_shifted(Bp[b], Bp[b + 1], t));
         const int k = wp::popc(ms);
         run += wp::popc(m0) - k; mst += k;
         if (run > best) { best = run; bb = b + 1; }
@@ -1361,8 +1371,8 @@ C2B_DEV int route_read(const KParams &P, DSmem &S, const RefDev &R, int r, const
     uint32_t m0w[2], msw[2];
 #pragma unroll
     for (int h = 0; h < 2; h++) {
-        m0w[h] = match(S.pl[0][w0 + h], S.pl[1][w0 + h]) & below(I - t1 - 32 * (w0 + h));
-        msw[h] = match(A1[w0 + h], shifted(B1[w0 + h], B1[w0 + h + 1], t1));
+        m0w[h] = pl_match(S.pl[0][w0 + h], S.pl[1][w0 + h]) & pl_below(I - t1 - 32 * (w0 + h));
+        msw[h] = pl_match(A1[w0 + h], pl_shifted(B1[w0 + h], B1[w0 + h + 1], t1));
     }
     // lane l: columns 2l, 2l + 1 of blocks w0, w0 + 1; F at the splits after them from F(32 w0) and a prefix sum over the lanes
     const int F0 = F1 - (wp::popc(m0w[0]) - wp::popc(msw[0]));
@@ -1387,43 +1397,95 @@ C2B_DEV int route_read(const KParams &P, DSmem &S, const RefDev &R, int r, const
 }
 
 // DG_PROVED if read rd is proved (op stream, meta word and classification written), else where it goes next (DG_KEEP: the
-// narrow tier, DG_ROUTE: straight to the wide ring; DG_KEEP whenever routing is off); all lanes call with warp-uniform arguments
-C2B_DEV int diag_read(const KParams &P, DSmem &S, int64_t rd, int64_t off, int J, int r, long long cnt, long long w, ScAcc<1> &A)
+// narrow tier, DG_ROUTE: straight to the wide ring; DG_KEEP whenever routing is off); all lanes call with warp-uniform arguments.
+// bytes: the read's J bytes (S.raw)
+C2B_DEV int diag_read(const KParams &P, DSmem &S, int64_t rd, const uint8_t *bytes, int J, int r, long long cnt, long long w,
+                      ScAcc<1> &A)
 {
     const int lane = wp::lane();
     const RefDev &R = refdev(P, r);
     const int I = R.I;
     // the reads the narrow tier would take (one candidate reference, packed ring admissible), of the amplicon's length
     if (!R.dg_ok || J != I || J > RG_COMBO || J + 32 > P.TS || J > R.pk_maxJ || I + J > PK_MAX_ALN) return DG_KEEP;
-    const bool bad = load_codes_a(P, S.lut, off, J, S.fw, S.rc);
+    const bool bad = load_codes_a(P, S.lut, bytes, J, S.fw, S.rc);
     wp::sync();
     // a symbol outside the alphabet or a seed test that wants both strands: the narrow tier only carries such a read to tier 2
     if (bad) return P.route ? DG_ROUTE : DG_KEEP;
     const int mode = strand_mode(P, R, S.fw, J);
     if (mode == 2) return P.route ? DG_ROUTE : DG_KEEP;     // both strands: the DP decides which one
     const uint8_t *c = mode == 1 ? S.rc : S.fw;
-    const int32_t *prof = R.prof;                    // [q][Ipad]: 4 x matrix[reference row][alphabet[q]]
-    const int Ipad = R.Ipad, dS = R.dg_S;
-    int acc[9];                                      // acc[s + 4]: 4 x ungapped score of read base k + s against reference row k
-#pragma unroll
-    for (int s = 0; s < 9; s++) acc[s] = 0;
-    for (int k = lane; k < I; k += 32) {
-        const int32_t *pk = prof + k;
-#pragma unroll
-        for (int s = -4; s <= 4; s++) {
-            const int j = k + s;
-            if ((s < 0 ? -s : s) <= dS && j >= 0 && j < J) acc[s + 4] += pk[(int)c[j] * Ipad];
+    // the read's bit planes in the aligned strand (lane b keeps word b; zero from word nb on) and, once per reference, the
+    // amplicon's: the popcount scores and route_read share them.  Either user implies I <= 256: 8 words and 2 zero words.
+    const int nb = (I + 31) >> 5, dS = R.dg_S;
+    uint4 rp = make_uint4(0u, 0u, 0u, 0u);
+    bool acgt = false;                               // every column of the read holds a code in 0..3
+    if (R.dg_two || R.rt_ok) {
+        for (int b = 0; b < nb; b++) {
+            const int x = 32 * b + lane, q = x < I ? c[x] : 255;
+            const uint32_t p0 = wp::ballot(q & 1), p1 = wp::ballot(q & 2), v = wp::ballot(q < 4);
+            if (lane == b) rp = make_uint4(p0, p1, v, 0u);
         }
+        acgt = wp::ballot(lane < nb && rp.z != pl_below(I - 32 * lane)) == 0;
+        if (lane < nb + 2) S.pl[0][lane] = rp;
+        const bool fresh = S.pl_ref != r;
+        wp::sync();
+        if (fresh) {
+            if (lane < nb + 2) S.pl[1][lane] = R.rt_pl[lane];
+            if (lane == 0) S.pl_ref = r;
+        }
+        wp::sync();
     }
+    int D;                                           // 4 x ungapped score on the main diagonal
+    bool proved;
+    if (R.dg_two && acgt) {
+        // every column scores dg_a4 (read code == amplicon code) or dg_b4: the same sums as below, grouped by the match
+        // counts of diagonal 0 and of offset s over its I - |s| columns (read base k + s against reference row k)
+        if (lane == 0) S.npop++;
+        const uint4 z4 = make_uint4(0u, 0u, 0u, 0u);
+        const uint4 rf = lane < nb ? S.pl[1][lane] : z4, rf1 = lane < nb ? S.pl[1][lane + 1] : z4, rp1 = lane < nb ? S.pl[0][lane + 1] : z4;
+        auto total = [](int v) {                     // over lanes 0..7 (the words), to every lane
 #pragma unroll
-    for (int s = 0; s < 9; s++)
+            for (int d = 4; d >= 1; d >>= 1) v += wp::shfl_xor(v, d);
+            return wp::shfl(v, 0);
+        };
+        const int m0 = total(wp::popc(pl_match(rp, rf)));
+        D = R.dg_a4 * m0 + R.dg_b4 * (I - m0);
+        proved = D > R.dg_thr4;
 #pragma unroll
-        for (int d = 16; d >= 1; d >>= 1) acc[s] += wp::shfl_xor(acc[s], d);
-    bool proved = acc[4] > R.dg_thr4;
+        for (int t = 1; t <= 4; t++) {
+            if (t > dS) break;
+            // offset +t: reference row x against read base x + t; offset -t: read base x against reference row x + t
+            const int m = total((wp::popc(pl_match(rf, pl_shifted(rp, rp1, t))) << 16) | wp::popc(pl_match(rp, pl_shifted(rf, rf1, t))));
+            const int mp = m >> 16, mn = m & 0xffff;
+            proved = proved && D > R.dg_a4 * mp + R.dg_b4 * (I - t - mp) + R.dg_c4[4 + t] &&
+                     D > R.dg_a4 * mn + R.dg_b4 * (I - t - mn) + R.dg_c4[4 - t];
+        }
+    } else {
+        const int32_t *prof = R.prof;                // [q][Ipad]: 4 x matrix[reference row][alphabet[q]]
+        const int Ipad = R.Ipad;
+        int acc[9];                                  // acc[s + 4]: 4 x ungapped score of read base k + s against reference row k
 #pragma unroll
-    for (int s = -4; s <= 4; s++)
-        if (s != 0 && (s < 0 ? -s : s) <= dS) proved = proved && acc[4] > acc[s + 4] + R.dg_c4[s + 4];
-    if (!proved) return P.route == 0 ? DG_KEEP : P.route == 2 ? DG_ROUTE : route_read(P, S, R, r, c, acc[4] >> 2);
+        for (int s = 0; s < 9; s++) acc[s] = 0;
+        for (int k = lane; k < I; k += 32) {
+            const int32_t *pk = prof + k;
+#pragma unroll
+            for (int s = -4; s <= 4; s++) {
+                const int j = k + s;
+                if ((s < 0 ? -s : s) <= dS && j >= 0 && j < J) acc[s + 4] += pk[(int)c[j] * Ipad];
+            }
+        }
+#pragma unroll
+        for (int s = 0; s < 9; s++)
+            if ((s < 4 ? 4 - s : s - 4) <= dS)
+#pragma unroll
+                for (int d = 16; d >= 1; d >>= 1) acc[s] += wp::shfl_xor(acc[s], d);
+        D = acc[4];
+        proved = D > R.dg_thr4;
+#pragma unroll
+        for (int s = -4; s <= 4; s++)
+            if (s != 0 && (s < 0 ? -s : s) <= dS) proved = proved && D > acc[s + 4] + R.dg_c4[s + 4];
+    }
+    if (!proved) return P.route == 0 ? DG_KEEP : P.route == 2 ? DG_ROUTE : route_read(R, S, D >> 2);
     // what align_narrow16 writes for an all-M traceback of I columns: op words of 32 ops, OP_NONE (3) past the end
     const int64_t slot = oslot(P, rd, r);
     if (lane < 16 && lane < P.NW) {
@@ -1431,15 +1493,31 @@ C2B_DEV int diag_read(const KParams &P, DSmem &S, int64_t rd, int64_t off, int J
         P.gops[slot * P.NW + lane] = rem >= 32 ? 0ull : rem <= 0 ? ~0ull : (~0ull << (2 * rem));
     }
     if (lane == 0) P.gmeta[slot] = gmeta_pack(I, mode == 1, GM_ALIGNED);
-    diag_classify(P, S, R, c, rd, r, mode == 1, cnt, w, A);
+    diag_classify(P, S, R, c, rd, r, mode == 1, cnt, w, A, R.dg_two && acgt);
     return DG_PROVED;
 }
 
 C2B_DEV void dsmem_init(const KParams &P, DSmem &S)
 {
     for (int k = wp::lane(); k < 256; k += 32) S.lut[k] = P.lut[k];
-    if (wp::lane() == 0) S.pl_ref = -1;
+    if (wp::lane() == 0) { S.pl_ref = -1; S.npop = 0; }
     wp::sync();
+}
+
+// Read x of the unit towards S.raw[b]: the 16-byte lines that hold its bytes (read byte p at S.raw[b][(address & 15) + p]),
+// copied in the background while the warp works on the read before it.  A line reaching past the read buffer is copied byte by
+// byte, nothing outside the buffer.  Reads longer than RG_COMBO are not copied: diag_read leaves them without looking.
+C2B_DEV void diag_stage(const KParams &P, DSmem &S, int x, int b)
+{
+    const int64_t off = S.off[x];
+    if (S.off[x + 1] - off > RG_COMBO) return;
+    const uint8_t *p0 = P.reads + off, *end = P.reads + S.off[x + 1], *lim = P.reads + S.total_bytes;
+    const int lane = wp::lane();
+    const uint8_t *wa = p0 - ((uintptr_t)p0 & 15) + 16 * lane;
+    uint8_t *dst = S.raw[b] + 16 * lane;
+    if (wa >= end) return;
+    if (wa >= P.reads && wa + 16 <= lim) wp::cp_async16(dst, wa);
+    else for (int k = 0; k < 16; k++) if (wa + k >= P.reads && wa + k < lim) dst[k] = wa[k];
 }
 
 // warp-aggregated append of reads first + x (bit x of mask) to a list: one atomic, the reads stay in order
@@ -1466,7 +1544,7 @@ C2B_DEV int diag_unit(const KParams &P, DSmem &S, int64_t u, ScAcc<1> &A, int &r
             S.off[lane] = P.offsets[rd]; S.ref[lane] = P.ref_id ? P.ref_id[rd] : 0;
             S.cnt[lane] = P.count ? P.count[rd] : 1; S.qw[lane] = P.qweight ? P.qweight[rd] : S.cnt[lane];
         }
-        if (lane == 0) S.off[n] = P.offsets[first + n];
+        if (lane == 0) { S.off[n] = P.offsets[first + n]; S.total_bytes = P.offsets[P.n_reads]; }
     }
     wp::sync();
 #ifndef C2B_EMU
@@ -1476,10 +1554,15 @@ C2B_DEV int diag_unit(const KParams &P, DSmem &S, int64_t u, ScAcc<1> &A, int &r
     }
 #endif
     uint32_t fail = 0, route = 0;
+    diag_stage(P, S, 0, 0);
 #pragma unroll 1
     for (int x = 0; x < n; x++) {
         const int64_t off = S.off[x];
-        const int v = diag_read(P, S, first + x, off, (int)(S.off[x + 1] - off), S.ref[x], S.cnt[x], S.qw[x], A);
+        wp::wait_async();
+        wp::sync();                                  // read x's bytes are in S.raw[x & 1]; read x + 1's go towards the other buffer
+        if (x + 1 < n) diag_stage(P, S, x + 1, (x + 1) & 1);
+        const int v = diag_read(P, S, first + x, S.raw[x & 1] + ((uintptr_t)(P.reads + off) & 15), (int)(S.off[x + 1] - off), S.ref[x],
+                                S.cnt[x], S.qw[x], A);
         if (v != DG_PROVED) fail |= 1u << x;
         if (v == DG_ROUTE) route |= 1u << x;
         wp::sync();
@@ -1515,6 +1598,7 @@ C2B_DEV void diag_loop(const KParams &P, DSmem &S, int64_t warp, int64_t nwarps)
         wp::addg(&wb.diag_proved, proved); wp::addg(&wb.diag_listed, seen - proved);
         wp::addg(&wb.tier2, routed);                    // tier-2 reads: routed here, and the narrow tier's failures
         wp::addg(&wb.routed, routed); wp::addg(&wb.kept, seen - proved - routed);
+        wp::addg(&wb.diag_popc, S.npop);
     }
 }
 

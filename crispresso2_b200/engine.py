@@ -300,5 +300,12 @@ class Engine:
         self._check(self.L.c2b_route_counts(self.h, C.byref(a), C.byref(b)), "c2b_route_counts")
         return a.value, b.value
 
+    def diag_popcount_reads(self):
+        """reads the diagonal tier scored by popcounts (a two-valued matrix over the amplicon, a read of A/C/G/T only)
+        since the last counts_reset"""
+        a = C.c_int64(0)
+        self._check(self.L.c2b_diag_popcount_reads(self.h, C.byref(a)), "c2b_diag_popcount_reads")
+        return a.value
+
     def launch_count(self):
         return int(self.L.c2b_launch_count(self.h))

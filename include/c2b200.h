@@ -264,6 +264,9 @@ int  c2b_diag_counts(c2b_engine *e, int64_t *proved, int64_t *tier1, int64_t *ti
 /* of the reads the diagonal tier did not prove since the last c2b_counts_reset: those it sent straight to the wide-ring
  * second tier (its routing test: C2B_NO_ROUTE switches it off) / those it kept for the narrow first tier */
 int  c2b_route_counts(c2b_engine *e, int64_t *routed, int64_t *kept);
+/* reads since the last c2b_counts_reset that the diagonal tier scored by popcounts of bit planes: reads of codes 0..3 against
+ * an amplicon of such codes whose scores over them are two-valued (a match score, a mismatch score) */
+int  c2b_diag_popcount_reads(c2b_engine *e, int64_t *reads);
 
 /* replaces: the count vectors / counters built by the quantification loop (CRISPRessoCORE.py:3841-3907,
  * :3964-4115).  Layout above.  c2b_counts_device exposes the block for an NCCL all-reduce.            */
