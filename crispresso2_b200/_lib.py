@@ -15,6 +15,7 @@ MAX_Q = 8
 MAX_SEEDS = 8
 MAX_READ_LEN = 512
 MAX_REF_LEN = 1024
+MAX_REFS = 32                                           # C2B_MAX_REFS: amplicons tried per read without a per-read ref_id
 
 F_IGNORE_SUBSTITUTIONS = 1
 F_IGNORE_INSERTIONS = 2

@@ -60,7 +60,7 @@ def _global_subs_quirk(st, src):
 def process_bam(bam_filename, bam_chr_loc, output_bam, variantCache, ref_names, refs, args, files_to_remove, output_directory,
                 engine=None, aln_matrix=None, on_out_of_contract="not_aligned"):
     """Drop-in for CRISPRessoCORE.process_bam (:2003-2280), single-process branch."""
-    core._unsupported(args, refs)
+    core._unsupported(args, refs, ref_names)
     if aln_matrix is None:
         loc = args.needleman_wunsch_aln_matrix_loc
         if not os.path.isabs(loc) and not os.path.exists(loc):

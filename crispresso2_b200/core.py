@@ -61,9 +61,12 @@ def _flags(args):
     return f
 
 
-def _unsupported(args, refs=None):
+def _unsupported(args, refs=None, ref_names=None):
     if getattr(args, "use_legacy_insertion_quantification", False) and refs and any(r.get("contains_coding_seq") for r in refs.values()):
         raise NotImplementedError("use_legacy_insertion_quantification together with a coding sequence is not built on the GPU path")
+    if ref_names is not None and len(ref_names) > _lib.MAX_REFS:
+        raise EngineError("%d amplicons: every read is tried against each of them, and the GPU path takes at most C2B_MAX_REFS = %d"
+                          % (len(ref_names), _lib.MAX_REFS))
 
 
 SCAFFOLD_REF, PE_REF = "Scaffold-incorporated", "Prime-edited"
@@ -464,7 +467,7 @@ def process_fastq(fastq_filename, variantCache, ref_names, refs, args, files_to_
     "not_aligned" (default) files them under not_aligned_variants with best_match_score -1 and logs their number; "error"
     raises EngineError before anything is launched."""
     from . import lazy
-    _unsupported(args, refs)
+    _unsupported(args, refs, ref_names)
     if aln_matrix is None:
         loc = args.needleman_wunsch_aln_matrix_loc
         if not os.path.isabs(loc) and not os.path.exists(loc):
@@ -689,7 +692,7 @@ def process_fastq_sharded(fastq_filename, variantCache, ref_names, refs, args, f
         return process_fastq(fastq_filename, variantCache, ref_names, refs, args, files_to_remove, output_directory,
                              engine=engine, aln_matrix=aln_matrix, on_out_of_contract=on_out_of_contract)
     from . import lazy
-    _unsupported(args, refs)
+    _unsupported(args, refs, ref_names)
     if aln_matrix is None:
         aln_matrix = read_matrix(args.needleman_wunsch_aln_matrix_loc)
     if engine is None:
@@ -727,7 +730,7 @@ def quantify(variantCache):
 
 
 def get_new_variant_object(args, fastq_seq, refs, ref_names, aln_matrix, pe_scaffold_dna_info=None, engine=None):
-    _unsupported(args, refs)
+    _unsupported(args, refs, ref_names)
     engine = engine or get_engine()
     configure_engine(engine, args, refs, ref_names, aln_matrix, edit_cap=max(len(refs[r]["sequence"]) for r in ref_names)
                      + len(fastq_seq) + 1)

@@ -1595,7 +1595,8 @@ int c2b_annotate_build(c2b_engine *e, const uint8_t *reads, const int64_t *offse
     for (int64_t k = 0; k < nb; k++) {
         if (label[k] < -1 || label[k] >= n_labels || aname[k] >= n_names) return fail(e, C2B_E_ARG, "c2b_annotate_build: label / name id out of range");
         if (amask[k] && label[k] < 0) return fail(e, C2B_E_ARG, "c2b_annotate_build: aligned read without a class label");
-        if (amask[k] >> R) return fail(e, C2B_E_ARG, "c2b_annotate_build: listed slot out of range");
+        // widened before the shift: a 32-bit shift by R = C2B_MAX_REFS = 32 is undefined (x86 shifts by 0 and refused every read)
+        if ((uint64_t)amask[k] >> R) return fail(e, C2B_E_ARG, "c2b_annotate_build: listed slot out of range");
         for (int r = 0; r < R; r++) {
             const uint32_t m = meta[k * R + r];
             if ((m >> 24) && ((int)(m & 0xffffu) > std::min(32 * NW, (int)C2B_MAX_ALN_LEN) || alns[k * R + r].n_edits > edit_cap))

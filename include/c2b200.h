@@ -106,7 +106,8 @@ typedef struct {
 
 /* Per read: best-reference selection of get_new_variant_object (CRISPRessoCORE.py:690-716, 780-785). 16 bytes */
 typedef struct {
-    uint32_t winner_mask;      /* bit r set: reference r is in best_match_names (before assign-first trimming) */
+    uint32_t winner_mask;      /* bit r set: reference r is in best_match_names (before assign-first trimming); under a
+                                  per-read ref_id (Pooled) the one candidate sets bit ref_id mod 32 */
     int32_t  best_score_milli; /* best_match_score*1000 ; <= 0: not aligned */
     int16_t  best_ref;         /* index of new_variant['best_match_name'] (last winner), -1 if none */
     uint8_t  n_winners;

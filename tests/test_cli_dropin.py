@@ -100,7 +100,17 @@ def _cases(tmp=None):
         pe_case.write_pairs(r1, r2, ns["FANC"])
         paired = ["-r1", r1, "-r2", r2, "-a", ns["FANC"], "-g", g, "--crispresso_merge",
                   "--fastp_command", sys.executable + " " + os.path.join(HERE, "fake_fastp.py")]
+    panel, names = allele_panel(ns["FANC"])
+    amas = ["-amas", "60,70,65,80,75"]
     return {
+        # five allele amplicons plus -e: six references per read, the one-kernel form of the general kernel
+        "fanc_panel": ["-r1", fq, "-a", ",".join(panel), "-an", ",".join(names), "-g", g, "-e", ns["FANC_HDR"],
+                       "--expand_ambiguous_alignments"] + amas,
+        "fanc_panel_fastq_output": ["-r1", fq, "-a", ",".join(panel), "-an", ",".join(names), "-g", g, "-e", ns["FANC_HDR"],
+                                    "--fastq_output"] + amas,
+        # the coding sequence lies in three of the five alleles: the other two carry a SNP inside it
+        "fanc_panel_coding": ["-r1", fq, "-a", ",".join(panel), "-an", ",".join(names), "-g", g,
+                              "-c", "GGGCCTTCGCGCACCTCATGGAATCCCTTCTGCAGCACCTGGATCGCTTTT"],
         # SURVEY 8(f) rank 3: --crispresso_merge, process_paired_fastq over one batch of GPU alignments (crispresso2_b200/paired.py)
         "fanc_paired_merge": paired,
         # (with -e the reference's own HDR re-projection fails on the paired entries' five-element ref_aln_details, :4243)
@@ -125,12 +135,22 @@ def _cases(tmp=None):
     }
 
 
+def allele_panel(fanc):
+    """five alleles of the FANC amplicon: itself and one SNP each at positions 30, 150, 60 and 100 (the last two inside the
+    coding sequence 56-107 of the fanc_params case, outside the guide 75-95) -> (sequences, names)"""
+    out = [fanc]
+    for p in (30, 150, 60, 100):
+        out.append(fanc[:p] + ("A" if fanc[p] != "A" else "C") + fanc[p + 1:])
+    return out, ["FANC", "SNP30", "SNP150", "SNP60", "SNP100"]
+
+
 SCORING_ARGS = ["--needleman_wunsch_aln_matrix_loc", os.path.join(HERE, "golden", "scoring_nuc.matrix"),
                 "--needleman_wunsch_gap_open", "-6", "--needleman_wunsch_gap_extend", "-6", "--needleman_wunsch_gap_incentive", "3"]
 
 
 @pytest.mark.parametrize("case", ["fanc_default", "fanc_params", "fanc_flags", "fanc_fastq_output", "fanc_legacy", "fanc_pe_scaffold",
-                                  "fanc_pe_scaffold_discard", "fanc_paired_merge", "fanc_paired_merge_out", "fanc_scoring"])
+                                  "fanc_pe_scaffold_discard", "fanc_paired_merge", "fanc_paired_merge_out", "fanc_scoring",
+                                  "fanc_panel", "fanc_panel_fastq_output", "fanc_panel_coding"])
 def test_reference_cli_with_engine_process_fastq_is_byte_identical(case, tmp_path):
     import build_emu
     lib = build_emu.build()

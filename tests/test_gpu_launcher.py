@@ -80,6 +80,26 @@ def _run_both(argv, tmp_path, env):
     return a
 
 
+def test_launcher_allele_panel(tmp_path):
+    """Five allele amplicons with -an names plus -e (six references per read: the general kernel alone, its phase sets in
+    step), --expand_ambiguous_alignments and a per-amplicon -amas, on the reference's FANC test FASTQ."""
+    from baseline import ref_shim
+    if not ref_shim.available():
+        pytest.skip("oracle/_ref/install (the pip-installed reference) was not built")
+    import pe_case
+    from test_cli_dropin import allele_panel
+    fq = str(tmp_path / "FANC.Cas9.fastq")
+    with open(fq, "w") as fh:
+        fh.write(pe_case.fanc_fastq_text())
+    import annotate_util as AU
+    fanc, fanc_hdr = AU.amplicons()
+    panel, names = allele_panel(fanc)
+    argv = ["-r1", fq, "-a", ",".join(panel), "-an", ",".join(names), "-g", "GGAATCCCTTCTGCAGCACC", "-e", fanc_hdr,
+            "--expand_ambiguous_alignments", "-amas", "60,70,65,80,75"]
+    snap = _run_both(argv, tmp_path, dict(os.environ, PYTHONPATH=ROOT))
+    assert len(snap) >= 10 and any("SNP150" in k for k in snap), sorted(snap)[:20]          # per-amplicon files written
+
+
 def test_launcher_prime_editing_scaffold(tmp_path):
     """'Scaffold-incorporated' re-labelling (CRISPRessoCORE.py:789-796) through the sm_90a library: the reads and pegRNA of the
     reference-generated fixture tests/golden/fanc_pe_scaffold.json.gz."""
