@@ -101,6 +101,11 @@ def _cases(tmp=None):
         paired = ["-r1", r1, "-r2", r2, "-a", ns["FANC"], "-g", g, "--crispresso_merge",
                   "--fastp_command", sys.executable + " " + os.path.join(HERE, "fake_fastp.py")]
     panel, names = allele_panel(ns["FANC"])
+    F = ns["FANC"]
+    win_fq, hdr_win = "", F[:118] + "TC" + F[118:128] + F[133:]          # 2-bp insertion inside 110-125, 128-132 deleted
+    if tmp is not None:
+        win_fq = window_fastq(os.path.join(str(tmp), "window_edges.fastq"), F)
+    g2 = F[150:170]
     amas = ["-amas", "60,70,65,80,75"]
     return {
         # five allele amplicons plus -e: six references per read, the one-kernel form of the general kernel
@@ -132,7 +137,30 @@ def _cases(tmp=None):
         "fanc_legacy": ["-r1", fq, "-a", ns["FANC"], "-g", g, "-e", ns["FANC_HDR"], "--use_legacy_insertion_quantification", "-w", "4"],
         # scoring options: an asymmetric NCBI-format matrix (tests/golden/scoring_nuc.matrix), gap_open == gap_extend, incentive 3
         "fanc_scoring": ["-r1", fq, "-a", ns["FANC"], "-g", g] + SCORING_ARGS,
+        # quantification windows (tests/test_window_space.py), reads with edits on every run edge: two guides, one with no
+        # window of its own (-w 5,0) and per-guide centres; three -qwc runs touching both ends, under legacy; -w 0; and -e
+        # with an HDR amplicon whose indels lie inside -qwc runs, so its cloned window differs from reference 0's
+        "window_two_guides": ["-r1", win_fq, "-a", F, "-g", g + "," + g2, "-w", "5,0", "--quantification_window_center=-3,-8"],
+        "window_qwc_ends_legacy": ["-r1", win_fq, "-a", F, "-g", g, "-qwc", "0-9_40-60_213-222", "--exclude_bp_from_left", "0",
+                                   "--exclude_bp_from_right", "0", "--use_legacy_insertion_quantification"],
+        "window_w0": ["-r1", win_fq, "-a", F, "-g", g, "-w", "0"],
+        "window_cloned_hdr": ["-r1", win_fq, "-a", F, "-g", g, "-e", hdr_win, "-qwc", "110-125_128-132"],
     }
+
+
+def window_fastq(path, fanc):
+    """the first 120 FANC reads, and reads with edits planted on the run edges of the windows of the window_* cases"""
+    import numpy as np
+    import pe_case
+    import test_window_space as WS
+    lines = pe_case.fanc_fastq_text().split("\n")
+    reads = [lines[k + 1] for k in range(0, len(lines) - 3, 4)][:120]
+    rng = np.random.default_rng(223)
+    for runs in ([(0, 9), (40, 60), (213, 222)], [(88, 97), (159, 168)], [(15, 207)], [(110, 125), (128, 132)]):
+        reads += WS.edge_reads(rng, fanc, runs)
+    with open(path, "w") as fh:
+        fh.write("".join("@r%d\n%s\n+\n%s\n" % (k, s, "I" * len(s)) for k, s in enumerate(reads)))
+    return path
 
 
 def allele_panel(fanc):
@@ -150,7 +178,8 @@ SCORING_ARGS = ["--needleman_wunsch_aln_matrix_loc", os.path.join(HERE, "golden"
 
 @pytest.mark.parametrize("case", ["fanc_default", "fanc_params", "fanc_flags", "fanc_fastq_output", "fanc_legacy", "fanc_pe_scaffold",
                                   "fanc_pe_scaffold_discard", "fanc_paired_merge", "fanc_paired_merge_out", "fanc_scoring",
-                                  "fanc_panel", "fanc_panel_fastq_output", "fanc_panel_coding"])
+                                  "fanc_panel", "fanc_panel_fastq_output", "fanc_panel_coding", "window_two_guides",
+                                  "window_qwc_ends_legacy", "window_w0", "window_cloned_hdr"])
 def test_reference_cli_with_engine_process_fastq_is_byte_identical(case, tmp_path):
     import build_emu
     lib = build_emu.build()

@@ -100,6 +100,18 @@ def test_launcher_allele_panel(tmp_path):
     assert len(snap) >= 10 and any("SNP150" in k for k in snap), sorted(snap)[:20]          # per-amplicon files written
 
 
+def test_launcher_window_runs_at_both_ends(tmp_path):
+    """-qwc of three runs, two of them touching position 0 and I - 1 (--exclude_bp_from_left / right 0), under
+    --use_legacy_insertion_quantification, on reads with edits planted on every run edge (tests/test_window_space.py)."""
+    from baseline import ref_shim
+    if not ref_shim.available():
+        pytest.skip("oracle/_ref/install (the pip-installed reference) was not built")
+    from test_cli_dropin import _cases
+    argv = _cases(tmp_path)["window_qwc_ends_legacy"]
+    snap = _run_both(argv, tmp_path, dict(os.environ, PYTHONPATH=ROOT))
+    assert len(snap) >= 10
+
+
 def test_launcher_prime_editing_scaffold(tmp_path):
     """'Scaffold-incorporated' re-labelling (CRISPRessoCORE.py:789-796) through the sm_90a library: the reads and pegRNA of the
     reference-generated fixture tests/golden/fanc_pe_scaffold.json.gz."""
