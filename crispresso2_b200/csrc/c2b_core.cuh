@@ -38,13 +38,9 @@ C2B_DEV uint32_t shflu_up(uint32_t v, int d) { return __shfl_up_sync(0xffffffffu
 C2B_DEV int shfl_xor(int v, int m) { return __shfl_xor_sync(0xffffffffu, v, m); }
 C2B_DEV uint32_t ballot(bool p) { return __ballot_sync(0xffffffffu, p); }
 C2B_DEV void sync() { __syncwarp(); }
-// barrier among the g warps of this warp's phase set (g consecutive warps): named barrier 1 + set index
-#ifdef C2B_X_INLINE_BARRIER
-C2B_DEV
-#else
-__device__ __noinline__        // ONE barrier instruction in the binary: every warp of a set waits at the same PC whatever path it is on
-#endif
-void grp_sync(int g)
+// barrier among the g warps of this warp's phase set (g consecutive warps): named barrier 1 + set index.  Out of line: ONE
+// barrier instruction in the binary, so every warp of a set waits at the same PC whatever path it is on
+__device__ __noinline__ void grp_sync(int g)
 {
     // g is a power of two: shifts, not the integer divisions that used to be inlined at every one of the dozen phase barriers
     const int w = (int)(threadIdx.x >> 5), sh = 31 - __clz(g);
@@ -538,9 +534,6 @@ C2B_DEV int score_milli(int m, int n)
 {
     // m <= n <= C2B_MAX_ALN_LEN = 1024: 100000*m < 2^27, so 32-bit unsigned arithmetic is exact (and the division is a
     // fraction of the 64-bit one's code)
-#ifdef C2B_DBG_DIV
-    if (n == 0) n = 1;
-#endif
     const uint32_t num = 100000u * (uint32_t)m, d = (uint32_t)n;
     uint32_t q = num / d; const uint32_t r = num - q * d;
     if (2u * r > d || (2u * r == d && (q & 1u))) q++;
@@ -798,15 +791,10 @@ C2B_DEVNOINL void coding_update(const KParams &P, const RefDev &R, const uint8_t
 
 // What only edited reads (or reads of a reference whose exons changed length) add to the count block once they are
 // counted: the size Counters (CRISPRessoCORE.py:4020-4043; the commonest bucket is implied, see c2b200.h), the
-// insertion/deletion/substitution class counters (:4022-4072) and the --coding_seq decision.  Out of line on purpose:
-// two thirds of the reads never get here and the per-read code must stay small (instruction cache).
-#ifdef C2B_X_NOINLINE_EDITED
-C2B_DEVNOINL
-#else
-C2B_DEV                       // inline: measured faster than the out-of-line call
-#endif
-void edited_update(const KParams &P, const RefDev &R, const uint8_t *rowinfo, const uint32_t *rowins,
-                                const RowOut &o, long long w)
+// insertion/deletion/substitution class counters (:4022-4072) and the --coding_seq decision.  Inline: measured faster than
+// an out-of-line call, although two thirds of the reads never get here.
+C2B_DEV void edited_update(const KParams &P, const RefDev &R, const uint8_t *rowinfo, const uint32_t *rowins,
+                           const RowOut &o, long long w)
 {
     const bool ign_s = P.flags & C2B_F_IGNORE_SUBSTITUTIONS, ign_i = P.flags & C2B_F_IGNORE_INSERTIONS,
                ign_d = P.flags & C2B_F_IGNORE_DELETIONS;
@@ -815,13 +803,11 @@ void edited_update(const KParams &P, const RefDev &R, const uint8_t *rowinfo, co
     const bool has_d = !ign_d && o.del_n > 0, has_i = !ign_i && o.ins_n > 0, has_s = !ign_s && o.sub_n > 0;
     unsigned long long *H = R.hist, *SC = R.scal;
     const int hs = P.hstride;
-#ifndef C2B_X_NOHIST
     if (has_i) wp::addg(H + (int64_t)C2B_H_INS_N * hs + o.ins_n, w);
     if (has_d) wp::addg(H + (int64_t)C2B_H_DEL_N * hs + o.del_n, w);
     if (has_s) wp::addg(H + (int64_t)C2B_H_SUB_N * hs + o.sub_n, w);
     const int eff = R.I + (has_i ? o.ins_n : 0) - (has_d ? o.del_n : 0);
     if (eff != R.I) wp::addg(H + (int64_t)C2B_H_EFF_LEN * hs + eff, w);
-#endif
     if (has_i) wp::addg(SC + C2B_S_INS, w);
     if (has_d) wp::addg(SC + C2B_S_DEL, w);
     if (has_s) wp::addg(SC + C2B_S_SUB, w);
@@ -917,14 +903,7 @@ C2B_DEV c2b_aln_rec load_aln(const c2b_aln_rec *p)
     return u.a;
 }
 
-#ifndef C2B_X_NOINLINE_SC
 C2B_DEV void sc_add(unsigned long long *SC, int slot, long long v) { wp::addg(SC + slot, v); }
-#else
-C2B_DEVNOINL void sc_add(unsigned long long *SC, int slot, long long v)
-{
-    if (v != 0) wp::addg(SC + slot, v);
-}
-#endif
 
 // Several references were tried: reload the op stream of the read's alignment to reference r (kept in opsbuf; lane offset
 // hoff >= 0: the stream lives in 16 lanes starting at hoff) and scatter it into the row-space view again.  -> irregular_ends
@@ -995,21 +974,6 @@ C2B_DEV void finish_read(const KParams &P, int64_t rd, c2b_read_rec rec, int J, 
                 else {
                     // the block of CRISPRessoCORE.py:4085-4171 is entered by modified reads, and by every read of a reference
                     // whose exons changed length (tot_exon_len_mod != 0)
-#ifdef C2B_X_BISECT_R01J      /* measurement only: the r01j body (no size Counters, no --coding_seq, no class deviation) */
-                    const bool lenv = modified && (o.n_ins_win > 0 || o.n_del_win > 0);
-                    if (two_scans || lenv) rows_run(P, R, rowinfo, rowins, o, nullptr, w, (two_scans ? RM_VEC : 0) | (lenv ? RM_LEN : 0));
-                    if (lane == 0) {
-                        wp::addg(SC + C2B_S_TOTAL, w);
-                        wp::addg(SC + (modified ? C2B_S_MODIFIED : C2B_S_UNMODIFIED), w);
-                        if (has_i) wp::addg(SC + C2B_S_INS, w);
-                        if (has_d) wp::addg(SC + C2B_S_DEL, w);
-                        if (has_s) wp::addg(SC + C2B_S_SUB, w);
-                        const int combo = (has_i ? 4 : 0) | (has_d ? 2 : 0) | (has_s ? 1 : 0);
-                        const int slot[8] = {-1, C2B_S_ONLY_SUB, C2B_S_ONLY_DEL, C2B_S_DEL_SUB, C2B_S_ONLY_INS, C2B_S_INS_SUB,
-                                             C2B_S_INS_DEL, C2B_S_INS_DEL_SUB};
-                        if (slot[combo] >= 0) wp::addg(SC + slot[combo], w);
-                    }
-#else
                     const bool entered = modified || R.tem != 0;
                     const bool lenv = entered && (o.n_ins_win > 0 || o.n_del_win > 0);
                     if (two_scans || lenv) rows_run(P, R, rowinfo, rowins, o, nullptr, w, (two_scans ? RM_VEC : 0) | (lenv ? RM_LEN : 0));
@@ -1018,18 +982,15 @@ C2B_DEV void finish_read(const KParams &P, int64_t rd, c2b_read_rec rec, int J, 
                         sc_add(SC, C2B_S_TOTAL, w);
                         sc_add(SC, modified ? C2B_S_MODIFIED : C2B_S_UNMODIFIED, w);
                     }
-#endif
                 }
             } else if (ambiguous && nth == 0 && w > 0 && lane == 0) sc_add(SC, C2B_S_AMBIGUOUS_W, w);
             // class_counts (:3984-3986) as a deviation from counts_modified / counts_unmodified: a discarded read still has
             // its class; a counted winner of an --expand_ambiguous_alignments read with several winners has a joined label
             // (derived on the host) instead
-#ifndef C2B_X_BISECT_R01J
             if (counted && lane == 0 && (two_scans || expand)) {
                 const bool discarded = two_scans && (o.del_n > 0 || o.ins_n > 0), joined = !ONE && expand && !first && rec.n_winners > 1;   // assign-first is tested first (:780-785)
                 if (discarded != joined) sc_add(SC, modified ? C2B_S_CLASS_MODIFIED : C2B_S_CLASS_UNMODIFIED, discarded ? w : -w);
             }
-#endif
             if (lane == 0) {
                 c2b_aln_rec a = multi ? load_aln(P.alns + oslot(P, rd, r)) : a_single;   // single reference: still in registers
                 a.insertion_n = (uint16_t)o.ins_n; a.deletion_n = (uint16_t)o.del_n; a.substitution_n = (uint16_t)o.sub_n;
@@ -1656,6 +1617,8 @@ C2B_DEV void process_quad(const KParams &P, WarpSmem &S, QuadSmem &Q, const uint
 // combined codes are built once (a pair qualifies only if every reference's seed test picks the same single strand), then
 // each reference in turn runs dp_ring over the same codes and its tracebacks, leaving the walked op streams in global
 // scratch (rgops); process_pair picks them up per reference and falls back to the full matrix where the band did not hold.
+// Kept apart from process_quad and out of line: folded into one inlined template, three amplicons with a coding sequence
+// ran 2 % slower (H100, DESIGN.md section 3).
 C2B_DEVNOINL void process_quad_multi(const KParams &P, WarpSmem &S, QuadSmem &Q, const uint32_t *staged_prof, int64_t first, int warp_slot)
 {
     const int lane = wp::lane(), g = lane >> 3;

@@ -125,24 +125,11 @@ static void rt_host_free(void *p) { free(p); }
 #endif
 
 // ----------------------------------------------------------------------------------------- kernel
-#ifndef C2B_WARPS_PER_CTA
-#define C2B_WARPS_PER_CTA 8
-#endif
-#ifndef C2B_MIN_CTAS_PER_SM
-#define C2B_MIN_CTAS_PER_SM 2
-#endif
-constexpr int WARPS_PER_CTA = C2B_WARPS_PER_CTA;      // general and ALIGN kernels
+constexpr int WARPS_PER_CTA = 8;                                 // general and ALIGN kernels
 static_assert(WARPS_PER_CTA % 4 == 0, "the general kernel's phase sets are four warps");
-#ifndef C2B_B_WARPS
-#define C2B_B_WARPS 4
-#endif
-constexpr int B_WARPS_PER_CTA = C2B_B_WARPS;                    // CLASSIFY kernel
-#ifndef C2B_B_MIN_CTAS
-#define C2B_B_MIN_CTAS 6
-#endif
-#ifndef C2B_A_MIN_CTAS
-#define C2B_A_MIN_CTAS 2
-#endif
+constexpr int MIN_CTAS_PER_SM = 2;                               // general kernel
+constexpr int A_MIN_CTAS = 2;                                    // ALIGN kernel
+constexpr int B_WARPS_PER_CTA = 4, B_MIN_CTAS = 6;               // CLASSIFY kernel
 constexpr int D_WARPS_PER_CTA = 8;                               // diagonal tier
 
 #ifndef C2B_EMU
@@ -177,7 +164,7 @@ __device__ __forceinline__ const uint32_t *stage_profile(const KParams &P, unsig
 // P is a __grid_constant__: the out-of-line device functions take it by reference, and without the qualifier every launch
 // copied the struct to each thread's local memory and read its fields back with LDL (slower).
 template <bool ONE>
-__global__ void __launch_bounds__(WARPS_PER_CTA * 32, C2B_MIN_CTAS_PER_SM) c2b_align_classify_kernel(const __grid_constant__ KParams P)
+__global__ void __launch_bounds__(WARPS_PER_CTA * 32, MIN_CTAS_PER_SM) c2b_align_classify_kernel(const __grid_constant__ KParams P)
 {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     WarpSmem *S = reinterpret_cast<WarpSmem *>(smem_raw) + (threadIdx.x >> 5);
@@ -192,7 +179,8 @@ __global__ void __launch_bounds__(WARPS_PER_CTA * 32, C2B_MIN_CTAS_PER_SM) c2b_a
     // ahead, so that the loop count -- and with it the number of barriers executed by process_group's phases -- is the same
     // for every warp of the set, and the next group's read bytes are on their way to L2 while this one computes.  This loop
     // needs the warps of a set in step, so it is the one loop the emulator does not share: it runs process_group per group
-    // there and checks the barrier count of each (run_plan).
+    // there and checks the barrier count of each (run_plan).  Free-running warps were measured 40-55 % slower on batches whose
+    // groups take the ring (DESIGN.md section 3).
     __shared__ unsigned long long next_base[WARPS_PER_CTA];
     const int gs = P.phase_sync, g = gs > 0 ? gs : 1, wib = threadIdx.x >> 5;
     const int set = wib / g, wis = wib % g;
@@ -224,7 +212,7 @@ __global__ void __launch_bounds__(WARPS_PER_CTA * 32, C2B_MIN_CTAS_PER_SM) c2b_a
 }
 
 // ALIGN kernel (c2b_split.cuh: align_loop)
-__global__ void __launch_bounds__(WARPS_PER_CTA * 32, C2B_A_MIN_CTAS) c2b_align_kernel(const __grid_constant__ KParams P)
+__global__ void __launch_bounds__(WARPS_PER_CTA * 32, A_MIN_CTAS) c2b_align_kernel(const __grid_constant__ KParams P)
 {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     ASmem *S = reinterpret_cast<ASmem *>(smem_raw) + (threadIdx.x >> 5);
@@ -242,7 +230,7 @@ __global__ void __launch_bounds__(D_WARPS_PER_CTA * 32) c2b_diag_kernel(const __
 
 // CLASSIFY kernel (c2b_split.cuh: classify_loop)
 template <bool ONE>
-__global__ void __launch_bounds__(B_WARPS_PER_CTA * 32, C2B_B_MIN_CTAS) c2b_classify_kernel(const __grid_constant__ KParams P)
+__global__ void __launch_bounds__(B_WARPS_PER_CTA * 32, B_MIN_CTAS) c2b_classify_kernel(const __grid_constant__ KParams P)
 {
     __shared__ BSmem smem[B_WARPS_PER_CTA];
     classify_loop<ONE>(P, smem[threadIdx.x >> 5], (int64_t)blockIdx.x * B_WARPS_PER_CTA + (threadIdx.x >> 5), (int64_t)gridDim.x * B_WARPS_PER_CTA);
@@ -379,7 +367,7 @@ int c2b_create(int device, c2b_engine **out)
     if (r == cudaSuccess) r = cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, device);
     if (r == cudaSuccess) r = cudaDeviceGetAttribute(&smem_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, device);
     if (r == cudaSuccess) r = cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device);
-    // room for a TMA-staged reference tile next to C2B_MIN_CTAS_PER_SM CTAs of per-warp state (1 KB per CTA is reserved by the driver)
+    // room for a TMA-staged reference tile next to MIN_CTAS_PER_SM CTAs of per-warp state (1 KB per CTA is reserved by the driver)
     // ... and the kernels' static shared memory (hand-out slots, mbarrier) -- if the sum is a byte too large the
     // occupancy query answers 1 CTA per SM and the persistent grid silently halves
     auto tile_room = [&](size_t per_warp, int ctas) {
@@ -389,7 +377,7 @@ int c2b_create(int device, c2b_engine **out)
         if (cap < 0) cap = 0;
         return cap & ~127;
     };
-    e->stage_cap = tile_room(sizeof(WarpSmem) + sizeof(QuadSmem), C2B_MIN_CTAS_PER_SM);
+    e->stage_cap = tile_room(sizeof(WarpSmem) + sizeof(QuadSmem), MIN_CTAS_PER_SM);
     const int dyn_smem = (int)((sizeof(WarpSmem) + sizeof(QuadSmem)) * WARPS_PER_CTA) + 128 + e->stage_cap;
     {
         const void *kernels[2] = {(const void *)c2b_align_classify_kernel<true>, (const void *)c2b_align_classify_kernel<false>};
@@ -403,7 +391,7 @@ int c2b_create(int device, c2b_engine **out)
     }
     // ALIGN kernel: its own (smaller) per-warp state; CTAs per SM from the occupancy query
     int occ_a = 0, occ_b = 0;
-    e->stage_cap_a = tile_room(sizeof(ASmem), C2B_A_MIN_CTAS);
+    e->stage_cap_a = tile_room(sizeof(ASmem), A_MIN_CTAS);
     const int dyn_a = (int)(sizeof(ASmem) * WARPS_PER_CTA) + 128 + e->stage_cap_a;
     if (r == cudaSuccess) r = cudaFuncSetAttribute((const void *)c2b_align_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dyn_a);
     if (r == cudaSuccess) r = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_a, (const void *)c2b_align_kernel, WARPS_PER_CTA * 32, dyn_a);
@@ -417,9 +405,9 @@ int c2b_create(int device, c2b_engine **out)
     if (occ < 1) occ = 1;
     if (occ_a < 1) occ_a = 1;
     if (occ_b < 1) occ_b = 1;
-    if (occ < C2B_MIN_CTAS_PER_SM)
-        fprintf(stderr, "[c2b] warning: only %d CTA(s) of the general kernel fit an SM (built for %d)\n", occ, C2B_MIN_CTAS_PER_SM);
-    if (occ_a > C2B_A_MIN_CTAS) occ_a = C2B_A_MIN_CTAS;
+    if (occ < MIN_CTAS_PER_SM)
+        fprintf(stderr, "[c2b] warning: only %d CTA(s) of the general kernel fit an SM (built for %d)\n", occ, MIN_CTAS_PER_SM);
+    if (occ_a > A_MIN_CTAS) occ_a = A_MIN_CTAS;
     e->grid = nsm * occ;                 // persistent: one wave of CTAs, warps pull work items from a counter
     e->grid_a = nsm * occ_a;
     e->grid_b = nsm * std::min(occ_b, 8);

@@ -5,11 +5,15 @@ time per launch of every kernel by name, the launch order of one step, the diago
 the card with its power limit: means over the profiled steps.
 
   python tools/kernel_times.py [--reads 1048576] [--steps 20] [--warmup 3] [--mix bench|proved|unproved] [--route-report] [--json OUT]
+  python tools/kernel_times.py --one-kernel coding1,coding3,amp8,nosplit [--reads 1048576] [--steps 20] [--warmup 3] [--json OUT]
 
 --mix replaces the bench's reads (same amplicon, same count): `proved` = reads as long as the amplicon with 0-2
 substitutions and no gap (what the diagonal tier proves), `unproved` = the bench's deletion and insertion templates only.
 --route-report repeats the steps with C2B_NO_ROUTE=1 and prints both kernel tables and the routing test's false-narrow reads
 (kept for the narrow tier, failed there) and false-wide reads (sent to the wide ring, would have passed the narrow tier).
+--one-kernel times the batches that launch the general kernel alone, one table per case: `coding1` = the bench amplicon with
+a coding sequence, `coding3` = the bench's three HDR-mode amplicons and reads with a coding sequence on the first, `amp8` =
+the bench amplicon and seven one-SNP alleles of it, `nosplit` = the bench batch under C2B_NO_SPLIT.
 """
 import argparse
 import json
@@ -53,6 +57,28 @@ def mix_reads(mix, ref, n):
     return out
 
 
+def one_kernel_case(case, n):
+    """-> (workload, launch switch to set or None) of a --one-kernel case: batches that launch the general kernel alone"""
+    from bench import Workload
+    from crispresso2_b200 import synth
+    w = Workload("hdr" if case == "coding3" else "single", n, 0)
+    if case in ("coding1", "coding3"):           # a coding sequence on the first amplicon: split_all is false
+        name = w.ref_names[0]
+        w.refs[name] = dict(w.refs[name], contains_coding_seq=True, exon_positions=list(range(40, 200)), splicing_positions=[],
+                            exon_len_mods=[0])
+        return w, None
+    if case == "amp8":                           # more than RG_MAX_REFS amplicons
+        amp = w.refs["Reference"]["sequence"]
+        for k in range(7):
+            p = 30 + 30 * k
+            w.refs["SNP%d" % k] = synth.amplicon_setup(amp[:p] + ("A" if amp[p] != "A" else "C") + amp[p + 1:])
+            w.ref_names.append("SNP%d" % k)
+        return w, None
+    if case == "nosplit":
+        return w, "C2B_NO_SPLIT"
+    raise SystemExit("kernel_times: unknown --one-kernel case %r" % case)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reads", type=int, default=1 << 20)
@@ -62,6 +88,8 @@ def main():
     ap.add_argument("--json", help="also write the table as JSON here")
     ap.add_argument("--route-report", action="store_true",
                     help="also run the steps with C2B_NO_ROUTE=1 and report the diagonal tier's false-narrow / false-wide routing")
+    ap.add_argument("--one-kernel", metavar="CASES",
+                    help="time the general kernel alone instead, for each of these comma-separated cases: coding1, coding3, amp8, nosplit")
     args = ap.parse_args()
 
     import numpy as np
@@ -74,29 +102,31 @@ def main():
     torch.cuda.set_device(0)
     dev = torch.device("cuda", 0)
     n = args.reads
-    w = Workload("single", n, 0)
     eng = Engine(0)
-    P = w.params
-    if args.mix != "bench":
-        w.buf = mix_reads(args.mix, w.refs["Reference"], n).reshape(-1)
-    eng.configure(w.refs, w.ref_names, O.make_matrix(), P.needleman_wunsch_gap_open, P.needleman_wunsch_gap_extend,
-                  P.aln_seed_count, P.aln_seed_min, w.flags, "ACGTN", 12)
-    W = eng.string_width(w.max_len)
     L = eng.L
-    d_reads = torch.from_numpy(np.ascontiguousarray(w.buf)).to(dev)
-    d_off = torch.from_numpy(w.off).to(dev)
-    d_recs = torch.empty(n * 16, dtype=torch.uint8, device=dev)
-    d_alns = torch.empty(n * 32, dtype=torch.uint8, device=dev)
-    d_str = torch.empty(n * 2 * W, dtype=torch.uint8, device=dev)
-    d_ed = torch.empty(n * 12 * 8, dtype=torch.uint8, device=dev)
 
-    def step():
-        rc = L.c2b_align_batch_device(eng.h, d_reads.data_ptr(), d_off.data_ptr(), n, w.max_len, None, None, None,
-                                      d_recs.data_ptr(), d_alns.data_ptr(), d_str.data_ptr(), d_ed.data_ptr())
-        if rc != 0:
-            raise RuntimeError(L.c2b_last_error(eng.h).decode())
+    def load(w):
+        """configure the engine for workload w and place its reads and outputs on the device -> one step"""
+        P = w.params
+        eng.configure(w.refs, w.ref_names, O.make_matrix(), P.needleman_wunsch_gap_open, P.needleman_wunsch_gap_extend,
+                      P.aln_seed_count, P.aln_seed_min, w.flags, "ACGTN", 12)
+        W = eng.string_width(w.max_len)
+        R = len(w.ref_names)
+        d_reads = torch.from_numpy(np.ascontiguousarray(w.buf)).to(dev)
+        d_off = torch.from_numpy(w.off).to(dev)
+        d_recs = torch.empty(n * 16, dtype=torch.uint8, device=dev)
+        d_alns = torch.empty(n * R * 32, dtype=torch.uint8, device=dev)
+        d_str = torch.empty(n * R * 2 * W, dtype=torch.uint8, device=dev)
+        d_ed = torch.empty(n * R * 12 * 8, dtype=torch.uint8, device=dev)
 
-    def measure():
+        def step():
+            rc = L.c2b_align_batch_device(eng.h, d_reads.data_ptr(), d_off.data_ptr(), n, w.max_len, None, None, None,
+                                          d_recs.data_ptr(), d_alns.data_ptr(), d_str.data_ptr(), d_ed.data_ptr())
+            if rc != 0:
+                raise RuntimeError(L.c2b_last_error(eng.h).decode())
+        return step
+
+    def measure(step):
         """-> (per-launch rows, sum, diag counts per step, route counts per step) of args.steps profiled steps"""
         for _ in range(args.warmup):
             eng.counts_reset()
@@ -153,7 +183,34 @@ def main():
             print("| %d | %s | %.3f | %.0f %% |" % (r["launch"], r["kernel"], r["ms_per_launch"], 100.0 * r["ms_per_launch"] / total if total else 0.0))
         print("| | sum of kernel times per step | %.3f | |" % total)
 
-    rows, total, diag, route = measure()
+    info = card_info(0)
+    if args.one_kernel:
+        cases = []
+        for case in args.one_kernel.split(","):
+            w, switch = one_kernel_case(case, n)
+            step = load(w)
+            if switch:
+                os.environ[switch] = "1"
+            try:
+                rows, total, _, _ = measure(step)
+            finally:
+                if switch:
+                    os.environ.pop(switch, None)
+            if len(rows) != 1:
+                raise SystemExit("kernel_times: --one-kernel %s launched %d kernels per step" % (case, len(rows)))
+            print("card: %s, power limit %s W; --one-kernel %s: %d reads x 250 bp, %d amplicons, %d profiled steps after %d warm-up "
+                  "steps" % (info.get("name"), info.get("power_limit_w"), case, n, len(w.ref_names), args.steps, args.warmup))
+            table(rows, total)
+            cases.append({"case": case, "amplicons": len(w.ref_names), "kernels": rows, "total_ms_per_step": total})
+        if args.json:
+            with open(args.json, "w") as fh:
+                json.dump({"card": info, "reads": n, "steps": args.steps, "one_kernel": cases}, fh, indent=1)
+        return
+    w = Workload("single", n, 0)
+    if args.mix != "bench":
+        w.buf = mix_reads(args.mix, w.refs["Reference"], n).reshape(-1)
+    step = load(w)
+    rows, total, diag, route = measure(step)
     report = None
     if args.route_report:
         # the same steps without routing: whether a read passes the narrow tier depends on the read alone, so the narrow
@@ -161,14 +218,13 @@ def main():
         # false-narrow = N_f (kept, then failed) and false-wide = N_r - (N0 - N_f) (routed, would have passed)
         os.environ["C2B_NO_ROUTE"] = "1"
         try:
-            rows0, total0, diag0, _ = measure()
+            rows0, total0, diag0, _ = measure(step)
         finally:
             os.environ.pop("C2B_NO_ROUTE", None)
         N0, Nr = diag0["tier2"], route["routed"]
         Nf = diag["tier2"] - Nr                          # tier-2 reads = routed + narrow failures
         report = {"listed": diag["tier1"], "N0": N0, "N_r": Nr, "N_f": Nf, "false_narrow": Nf, "false_wide": Nr - (N0 - Nf),
                   "kernels_no_route": rows0, "total_ms_no_route": total0}
-    info = card_info(0)
     print("card: %s, power limit %s W, max SM clock %s MHz" % (info.get("name"), info.get("power_limit_w"), info.get("max_sm_clock_mhz")))
     print("%d reads x 250 bp (mix %s), %d profiled steps after %d warm-up steps; C2B_NO_DIAG=%s" % (
         n, args.mix, args.steps, args.warmup, os.environ.get("C2B_NO_DIAG", "")))
