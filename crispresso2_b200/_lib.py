@@ -35,6 +35,7 @@ ST_UNDEFINED = 2
 ST_EDIT_OVERFLOW = 4
 E_ARG, E_LIMIT, E_STATE = -2, -3, -4                    # C2B_E_* of include/c2b200.h
 ST_TOO_LONG = 8
+VCF_E_KEY, VCF_E_NOT_IN_LIST, VCF_E_STRING_INDEX, VCF_E_EMPTY_MAX = 1, 2, 3, 4     # C2B_VCF_E_*: c2b_vcf_edit_counts' err[1]
 
 # count-block layout (enum order of c2b200.h)
 V_ALL_INS, V_ALL_INS_LEFT, V_ALL_DEL, V_ALL_SUB, V_INS, V_DEL, V_SUB, V_SUBBASE0 = range(8)
@@ -92,7 +93,8 @@ EXPORTS = ["c2b_create", "c2b_destroy", "c2b_last_error", "c2b_configure", "c2b_
            "c2b_annotate_build", "c2b_annotate_free", "c2b_annotate_n", "c2b_annotate_arena", "c2b_annotate_offsets",
            "c2b_annotate_cigar_arena", "c2b_annotate_cigar_offsets", "c2b_annotate_flags", "c2b_annotate_mapq", "c2b_annotate_first",
            "c2b_annotate_last_record", "c2b_annotate_record_arena", "c2b_annotate_record_offsets", "c2b_annotate_write_fastq",
-           "c2b_annotate_write_sam", "c2b_annotate_write_sam_passthrough"]
+           "c2b_annotate_write_sam", "c2b_annotate_write_sam_passthrough", "c2b_vcf_edit_counts", "c2b_vcf_free", "c2b_vcf_n",
+           "c2b_vcf_keys", "c2b_vcf_key_offsets", "c2b_vcf_reads", "c2b_vcf_n_records", "c2b_vcf_timings"]
 
 _cache = {}
 
@@ -256,5 +258,15 @@ def load(path=None):
     L.c2b_annotate_write_sam.argtypes = [vp, vp, vp, i64, C.c_char_p, C.c_char_p, C.c_char_p, i32, cpp, cpp, vp, i32]
     L.c2b_annotate_write_sam_passthrough.restype = C.c_int
     L.c2b_annotate_write_sam_passthrough.argtypes = [vp, vp, vp, i64, vp, C.c_size_t, C.c_char_p, i32]
+    L.c2b_vcf_edit_counts.restype = C.c_int
+    L.c2b_vcf_edit_counts.argtypes = [vp, i64] + [vp] * 17 + [i64, vp, C.POINTER(vp)]
+    L.c2b_vcf_free.restype = None
+    L.c2b_vcf_free.argtypes = [vp]
+    for name, rt in (("c2b_vcf_n", i64), ("c2b_vcf_keys", vp), ("c2b_vcf_key_offsets", vp), ("c2b_vcf_reads", vp),
+                     ("c2b_vcf_n_records", i64)):
+        getattr(L, name).restype = rt
+        getattr(L, name).argtypes = [vp]
+    L.c2b_vcf_timings.restype = C.c_int
+    L.c2b_vcf_timings.argtypes = [vp, C.POINTER(C.c_double), C.POINTER(C.c_double)]
     _cache[path] = L
     return L

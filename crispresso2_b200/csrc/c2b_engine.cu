@@ -24,6 +24,7 @@
 #include "c2b_core.cuh"
 #include "c2b_split.cuh"
 #include "c2b_annotate.cuh"
+#include "c2b_vcf.cuh"
 #include "c2b_fastq_int.h"
 
 using namespace c2b;
@@ -1729,6 +1730,162 @@ const int16_t *c2b_annotate_first(const c2b_annotation *a) { return a ? a->first
 const int64_t *c2b_annotate_last_record(const c2b_annotation *a) { return a && !a->last_rec.empty() ? a->last_rec.data() : nullptr; }
 const uint8_t *c2b_annotate_record_arena(const c2b_annotation *a) { return a ? (const uint8_t *)a->rec.data() : nullptr; }
 const int64_t *c2b_annotate_record_offsets(const c2b_annotation *a) { return a && !a->rec_off.empty() ? a->rec_off.data() : nullptr; }
+
+// --vcf_output edit counts (c2b_vcf.cuh) for packed allele rows in chunks: the chunk's rows go up through one pinned buffer, a
+// size pass notes every row's records, bytes and first exception, a scan places them, a write pass builds the records, which
+// come back through a second pinned buffer.  The records of all chunks are then summed on the host (c2b_vcf_sum_records).
+int c2b_vcf_edit_counts(c2b_engine *e, int64_t n_rows, const int32_t *chrom, const int64_t *pos, const int64_t *reads,
+                        const uint8_t *ref, const int64_t *ref_off, const uint8_t *aln, const int64_t *aln_off,
+                        const int64_t *rp, const int64_t *rp_off, const int64_t *del, const int64_t *del_off,
+                        const int64_t *ins, const int64_t *ins_off, const int64_t *isz, const int64_t *isz_off,
+                        const int64_t *sub, const int64_t *sub_off, int64_t chunk, int64_t *err, c2b_vcf_counts **out)
+{
+    if (!e || !out || !err || n_rows < 0 || !ref_off || !aln_off || !rp_off || !del_off || !ins_off || !isz_off || !sub_off)
+        return fail(e, C2B_E_ARG, "c2b_vcf_edit_counts: bad argument");
+    *out = nullptr;
+    err[0] = -1; err[1] = 0; err[2] = 0;
+    const int64_t *offs[7] = {ref_off, aln_off, rp_off, del_off, ins_off, isz_off, sub_off};
+    for (const int64_t *o : offs) {
+        if (o[0] != 0) return fail(e, C2B_E_ARG, "c2b_vcf_edit_counts: offsets must start at 0");
+        for (int64_t r = 0; r < n_rows; r++) if (o[r + 1] < o[r]) return fail(e, C2B_E_ARG, "c2b_vcf_edit_counts: offsets must not decrease");
+    }
+    if (n_rows && (!chrom || !pos || !reads || (ref_off[n_rows] && !ref) || (aln_off[n_rows] && !aln) || (rp_off[n_rows] && !rp) ||
+                   (del_off[n_rows] && !del) || (ins_off[n_rows] && !ins) || (isz_off[n_rows] && !isz) || (sub_off[n_rows] && !sub)))
+        return fail(e, C2B_E_ARG, "c2b_vcf_edit_counts: row arrays missing");
+    if (chunk <= 0) chunk = 1 << 14;
+    const auto t0 = std::chrono::steady_clock::now();
+    auto al = [](size_t x) { return (x + 255) & ~(size_t)255; };
+    DevBuf d_in, d_len, d_out;
+    uint8_t *h_in = nullptr, *h_out = nullptr; size_t h_in_cap = 0, h_out_cap = 0;
+    auto cleanup = [&]() { rt_free(d_in.p); rt_free(d_len.p); rt_free(d_out.p); rt_host_free(h_in); rt_host_free(h_out); };
+    auto grow_host = [](uint8_t *&p, size_t &cap, size_t n) {
+        if (n <= cap) return true;
+        rt_host_free(p); cap = n + n / 4 + 4096; p = (uint8_t *)rt_host_alloc(cap);
+        return p != nullptr;
+    };
+    std::vector<uint8_t> keys;                                   // every record of every chunk, in row order
+    std::vector<int64_t> rec_pos, rec_w;
+    auto one_chunk = [&](int64_t r0) -> int {
+        const int64_t r1 = std::min(n_rows, r0 + chunk), m = r1 - r0;
+        // chunk input layout (device): chrom | pos | reads | then per column its values and its offsets rebased to the chunk
+        const void *col[7] = {ref, aln, rp, del, ins, isz, sub};
+        const size_t width[7] = {1, 1, 8, 16, 16, 8, 8};
+        size_t o_chrom = 0, o_pos = al((size_t)m * 4), o_reads = o_pos + al((size_t)m * 8), o = o_reads + al((size_t)m * 8);
+        size_t o_val[7], o_off[7];
+        for (int c = 0; c < 7; c++) {
+            o_val[c] = o; o += al((size_t)(offs[c][r1] - offs[c][r0]) * width[c]);
+            o_off[c] = o; o += al((size_t)(m + 1) * 8);
+        }
+        const size_t o_end = o;
+        if (!grow_host(h_in, h_in_cap, o_end)) return fail(e, C2B_E_CUDA, "c2b_vcf_edit_counts: pinned allocation");
+        memcpy(h_in + o_chrom, chrom + r0, (size_t)m * 4);
+        memcpy(h_in + o_pos, pos + r0, (size_t)m * 8);
+        memcpy(h_in + o_reads, reads + r0, (size_t)m * 8);
+        for (int c = 0; c < 7; c++) {
+            const int64_t b = offs[c][r0];
+            const size_t nb = (size_t)(offs[c][r1] - b) * width[c];
+            if (nb) memcpy(h_in + o_val[c], (const uint8_t *)col[c] + (size_t)b * width[c], nb);
+            int64_t *ho = (int64_t *)(h_in + o_off[c]);
+            for (int64_t r = 0; r <= m; r++) ho[r] = offs[c][r0 + r] - b;
+        }
+        // per row: nrec | nbytes | err (2) | rec_base (m + 1) | key_off (m + 1) | first (3)
+        const size_t l_nrec = 0, l_nbytes = al((size_t)m * 8), l_err = l_nbytes + al((size_t)m * 8), l_rb = l_err + al((size_t)m * 16),
+                     l_ko = l_rb + al((size_t)(m + 1) * 8), l_first = l_ko + al((size_t)(m + 1) * 8), l_end = l_first + 3 * 8;
+        int rc2;
+        if ((rc2 = ensure(e, d_in, o_end)) || (rc2 = ensure(e, d_len, l_end))) return rc2;
+        RTCHK(rt_h2d(d_in.p, h_in, o_end, e->stream));
+        char *di = (char *)d_in.p, *dl = (char *)d_len.p;
+        c2b::vcf::VParams P;
+        memset(&P, 0, sizeof P);
+        P.n = m;
+        P.chrom = (const int32_t *)(di + o_chrom); P.pos = (const int64_t *)(di + o_pos); P.reads = (const int64_t *)(di + o_reads);
+        P.ref = (const uint8_t *)(di + o_val[0]); P.ref_off = (const int64_t *)(di + o_off[0]);
+        P.aln = (const uint8_t *)(di + o_val[1]); P.aln_off = (const int64_t *)(di + o_off[1]);
+        P.rp = (const int64_t *)(di + o_val[2]); P.rp_off = (const int64_t *)(di + o_off[2]);
+        P.del = (const int64_t *)(di + o_val[3]); P.del_off = (const int64_t *)(di + o_off[3]);
+        P.ins = (const int64_t *)(di + o_val[4]); P.ins_off = (const int64_t *)(di + o_off[4]);
+        P.isz = (const int64_t *)(di + o_val[5]); P.isz_off = (const int64_t *)(di + o_off[5]);
+        P.sub = (const int64_t *)(di + o_val[6]); P.sub_off = (const int64_t *)(di + o_off[6]);
+        P.nrec = (int64_t *)(dl + l_nrec); P.nbytes = (int64_t *)(dl + l_nbytes); P.err = (int64_t *)(dl + l_err);
+        P.rec_base = (const int64_t *)(dl + l_rb); P.key_off = (const int64_t *)(dl + l_ko);
+        int64_t first[3] = {-1, 0, 0}, tot[2] = {0, 0};
+#ifndef C2B_EMU
+        const int grid = (int)std::min<int64_t>((m + 7) / 8, 8192);
+        c2b_vcf_size_kernel<<<grid, 256, 0, e->stream>>>(P);
+        c2b_vcf_scan_kernel<<<1, 32, 0, e->stream>>>(P.nrec, (int64_t *)P.rec_base, P.nbytes, (int64_t *)P.key_off, P.err,
+                                                     (int64_t *)(dl + l_first), m);
+        RTCHK(cudaGetLastError());
+        RTCHK(rt_d2h(first, dl + l_first, 24, e->stream));
+        RTCHK(rt_d2h(&tot[0], P.rec_base + m, 8, e->stream));
+        RTCHK(rt_d2h(&tot[1], P.key_off + m, 8, e->stream));
+        RTCHK(rt_sync(e->stream));
+#else
+        for (int64_t r = 0; r < m; r++) emu::run_warp([&]() { c2b::vcf::edits_one<false>(P, r); });
+        emu::run_warp([&]() {
+            c2b::ann::scan_sizes(P.nrec, (int64_t *)P.rec_base, m);
+            c2b::ann::scan_sizes(P.nbytes, (int64_t *)P.key_off, m);
+            c2b::vcf::first_error(P.err, m, (int64_t *)(dl + l_first));
+        });
+        memcpy(first, dl + l_first, 24);
+        tot[0] = P.rec_base[m]; tot[1] = P.key_off[m];
+#endif
+        if (first[0] >= 0) {
+            static const char *what[5] = {"", "KeyError", "ValueError: value is not in list", "IndexError: string index out of range",
+                                          "ValueError: max() iterable argument is empty"};
+            err[0] = r0 + first[0]; err[1] = first[1]; err[2] = first[2];
+            char msg[160];
+            snprintf(msg, sizeof msg, "c2b_vcf_edit_counts: row %lld raises %s (value %lld)", (long long)err[0],
+                     what[first[1] >= 1 && first[1] <= 4 ? first[1] : 0], (long long)err[2]);
+            return fail(e, C2B_E_ARG, msg);
+        }
+        const size_t o_keys = 0, o_rpos = al((size_t)tot[1]), o_rw = o_rpos + al((size_t)tot[0] * 8), out_end = o_rw + (size_t)tot[0] * 8;
+        if ((rc2 = ensure(e, d_out, out_end + 16))) return rc2;
+        char *dout = (char *)d_out.p;
+        P.keys = (uint8_t *)(dout + o_keys); P.rec_pos = (int64_t *)(dout + o_rpos); P.rec_w = (int64_t *)(dout + o_rw);
+#ifndef C2B_EMU
+        c2b_vcf_write_kernel<<<grid, 256, 0, e->stream>>>(P);
+        RTCHK(cudaGetLastError());
+#else
+        for (int64_t r = 0; r < m; r++) emu::run_warp([&]() { c2b::vcf::edits_one<true>(P, r); });
+#endif
+        if (!grow_host(h_out, h_out_cap, out_end)) return fail(e, C2B_E_CUDA, "c2b_vcf_edit_counts: pinned allocation");
+        RTCHK(rt_d2h(h_out, dout, out_end, e->stream));
+        RTCHK(rt_sync(e->stream));
+        const int64_t kb = (int64_t)keys.size();
+        keys.insert(keys.end(), h_out + o_keys, h_out + o_keys + tot[1]);
+        const int64_t *hp = (const int64_t *)(h_out + o_rpos), *hw = (const int64_t *)(h_out + o_rw);
+        for (int64_t i = 0; i < tot[0]; i++) rec_pos.push_back(kb + hp[i]);
+        rec_w.insert(rec_w.end(), hw, hw + tot[0]);
+        return C2B_OK;
+    };
+    int rc = C2B_OK;
+    for (int64_t r0 = 0; !rc && r0 < n_rows; r0 += chunk) rc = one_chunk(r0);
+    cleanup();
+    if (rc) return rc;
+    const auto t1 = std::chrono::steady_clock::now();
+    rec_pos.push_back((int64_t)keys.size());
+    std::unique_ptr<c2b_vcf_counts> V(new c2b_vcf_counts());
+    if (!c2b_vcf_sum_records(keys.data(), rec_pos.data(), rec_w.data(), (int64_t)rec_w.size(), V.get()))
+        return fail(e, C2B_E_LIMIT, "c2b_vcf_edit_counts: a summed #Reads leaves int64");
+    const auto t2 = std::chrono::steady_clock::now();
+    V->device_ms = std::chrono::duration<double, std::milli>(t1 - t0).count();
+    V->sum_ms = std::chrono::duration<double, std::milli>(t2 - t1).count();
+    *out = V.release();
+    return C2B_OK;
+}
+
+void c2b_vcf_free(c2b_vcf_counts *v) { delete v; }
+int64_t c2b_vcf_n(const c2b_vcf_counts *v) { return v ? (int64_t)v->reads.size() : 0; }
+const uint8_t *c2b_vcf_keys(const c2b_vcf_counts *v) { return v ? v->keys.get() : nullptr; }
+const int64_t *c2b_vcf_key_offsets(const c2b_vcf_counts *v) { return v ? v->key_off.data() : nullptr; }
+const int64_t *c2b_vcf_reads(const c2b_vcf_counts *v) { return v ? v->reads.data() : nullptr; }
+int64_t c2b_vcf_n_records(const c2b_vcf_counts *v) { return v ? v->n_records : 0; }
+int c2b_vcf_timings(const c2b_vcf_counts *v, double *device_ms, double *sum_ms)
+{
+    if (!v || !device_ms || !sum_ms) return C2B_E_ARG;
+    *device_ms = v->device_ms; *sum_ms = v->sum_ms;
+    return C2B_OK;
+}
 
 // pinned host memory for callers that want full-speed copies (bench.py, the Python wrapper)
 void *c2b_host_alloc(size_t n)

@@ -221,12 +221,14 @@ bool read_gz(const char *path, c2b_bytes &buf, std::string &err)
 }
 
 // (3) sharded exact dedup in file order and (4) the unique reads in first-seen order, from every record's sequence and hash:
-// shared by the FASTQ front end and the SAM one (c2b_sam_dedup_buffer)
+// shared by the FASTQ front end, the SAM one (c2b_sam_dedup_buffer) and the VCF edit counts (c2b_vcf_sum_records: with
+// `weight`, each unique's sum of its records' weights goes to sums[u]; *overflow is set when one leaves int64)
 void dedup_records(const std::vector<Seq> &seq, const std::vector<uint64_t> &hv, int64_t n_rec, int T, c2b_fastq *F,
-                   const std::function<void(const char *)> &lap)
+                   const std::function<void(const char *)> &lap, const int64_t *weight = nullptr,
+                   std::vector<int64_t> *sums = nullptr, std::atomic<bool> *overflow = nullptr)
 {
     // (3) sharded exact dedup in file order
-    struct Ent { int64_t first; int32_t count; };
+    struct Ent { int64_t first; int32_t count; int64_t sum; };
     std::vector<std::vector<Ent>> found(T);
     auto shard = [&](int s) {
         size_t mine = 0;
@@ -241,9 +243,13 @@ void dedup_records(const std::vector<Seq> &seq, const std::vector<uint64_t> &hv,
             size_t k = (size_t)h & (cap - 1);
             for (;;) {
                 const int32_t e = slot[k];
-                if (e < 0) { slot[k] = (int32_t)E.size(); E.push_back({r, 1}); break; }
+                if (e < 0) { slot[k] = (int32_t)E.size(); E.push_back({r, 1, weight ? weight[r] : 0}); break; }
                 const Seq &a = seq[(size_t)E[(size_t)e].first], &b = seq[(size_t)r];
-                if (hv[(size_t)E[(size_t)e].first] == h && a.len == b.len && memcmp(a.p, b.p, a.len) == 0) { E[(size_t)e].count++; break; }
+                if (hv[(size_t)E[(size_t)e].first] == h && a.len == b.len && memcmp(a.p, b.p, a.len) == 0) {
+                    E[(size_t)e].count++;
+                    if (weight && __builtin_add_overflow(E[(size_t)e].sum, weight[r], &E[(size_t)e].sum)) overflow->store(true);
+                    break;
+                }
                 k = (k + 1) & (cap - 1);
             }
         }
@@ -259,8 +265,11 @@ void dedup_records(const std::vector<Seq> &seq, const std::vector<uint64_t> &hv,
     // (4) unique reads in first-seen order: the shards' entries are scattered to their first record (disjoint records, so
     // in parallel), a prefix count over the records numbers them -- no sort, no serial pass over the unique reads
     std::vector<int32_t> cnt_at((size_t)n_rec, 0);
+    std::vector<int64_t> sum_at(weight ? (size_t)n_rec : 0);
     {
-        auto scatter = [&](int t) { for (const Ent &e : found[(size_t)t]) cnt_at[(size_t)e.first] = e.count; };
+        auto scatter = [&](int t) {
+            for (const Ent &e : found[(size_t)t]) { cnt_at[(size_t)e.first] = e.count; if (weight) sum_at[(size_t)e.first] = e.sum; }
+        };
         std::vector<std::thread> th;
         for (int t = 1; t < T; t++) th.emplace_back(scatter, t);
         scatter(0);
@@ -289,6 +298,7 @@ void dedup_records(const std::vector<Seq> &seq, const std::vector<uint64_t> &hv,
     F->first_index.resize(nu);
     F->offsets[nu] = tot;
     F->seqs.reset(new uint8_t[(size_t)tot + 16]);
+    if (weight) sums->resize(nu);
     {
         auto emit = [&](int t) {
             size_t u = u0[(size_t)t]; int64_t by = b0[(size_t)t];
@@ -297,6 +307,7 @@ void dedup_records(const std::vector<Seq> &seq, const std::vector<uint64_t> &hv,
                 if (!c) continue;
                 const Seq &q = seq[(size_t)r];
                 F->offsets[u] = by; F->counts[u] = c; F->first_index[u] = r;
+                if (weight) (*sums)[u] = sum_at[(size_t)r];
                 memcpy(F->seqs.get() + by, q.p, q.len);
                 by += q.len; u++;
             }
@@ -310,6 +321,26 @@ void dedup_records(const std::vector<Seq> &seq, const std::vector<uint64_t> &hv,
 }
 
 }  // namespace
+
+bool c2b_vcf_sum_records(const uint8_t *arena, const int64_t *off, const int64_t *w, int64_t n, c2b_vcf_counts *out)
+{
+    std::vector<Seq> seq((size_t)n);
+    std::vector<uint64_t> hv((size_t)n);
+    const int T = host_threads((size_t)(n ? off[n] - off[0] : 0));
+    run_threads(T, [&](int t) {
+        for (int64_t i = n * t / T; i < n * (t + 1) / T; i++) {
+            seq[(size_t)i] = {arena + off[i], (uint32_t)(off[i + 1] - off[i])};
+            hv[(size_t)i] = hash_bytes(arena + off[i], (size_t)(off[i + 1] - off[i]));
+        }
+    });
+    c2b_fastq F;
+    std::atomic<bool> overflow(false);
+    dedup_records(seq, hv, n, T, &F, [](const char *) {}, w, &out->reads, &overflow);
+    out->keys = std::move(F.seqs);
+    out->key_off = std::move(F.offsets);
+    out->n_records = n;
+    return !overflow.load();
+}
 
 static std::string g_fastq_err;
 

@@ -40,6 +40,18 @@ struct c2b_annotation {
     std::string rec;
 };
 
+// --vcf_output edit counts (built by c2b_vcf_edit_counts in c2b_engine.cu): the distinct record keys in first-seen order, key i
+// at keys[key_off[i] .. key_off[i+1]), and the summed #Reads of each
+struct c2b_vcf_counts {
+    std::unique_ptr<uint8_t[]> keys;
+    std::vector<int64_t> key_off, reads;
+    int64_t n_records = 0;
+    double device_ms = 0, sum_ms = 0;
+};
+// the records rec[i] = arena[off[i] .. off[i+1]) with weights w[i], equal records summed (the exact hash of the FASTQ front end);
+// false when a sum leaves int64
+bool c2b_vcf_sum_records(const uint8_t *arena, const int64_t *off, const int64_t *w, int64_t n, c2b_vcf_counts *out);
+
 // whole file into memory (c2b_fastq.cpp): plain read / gzip inflate (blocked gzip: all host threads)
 bool c2b_fastq_read_gz(const char *path, c2b_bytes &buf, std::string &err);
 void c2b_fastq_set_error(const std::string &m);

@@ -16,6 +16,9 @@ What is re-bound (INTEGRATION.md section 2), nothing else of the reference chang
   * filterFastqs.filterFastqs (imported and called at CRISPRessoCORE.py:3716-3717)          -> crispresso2_b200.filter_fastqs.filterFastqs
   * CRISPRessoShared.get_dataframe_around_cut_asymmetrical (plots/data_prep.py:1537)        -> the native grouping of
     crispresso2_b200.alleles when the frame was built by AlleleTable.to_dataframe(), the reference's own function otherwise.
+  * writers.vcf.build_edit_counts (module global, called by vcf.write_vcf_file, writers/vcf.py:317; --vcf_output,
+    CRISPRessoCORE.py:4487-4496)   -> crispresso2_b200.vcf.build_edit_counts on the launcher's engine, in single-process runs
+    and under torchrun alike (every rank runs main() over the same cache)
 Under torchrun (WORLD_SIZE > 1) every rank runs the same command; process_fastq shards the unique reads over the ranks' GPUs
 and merges the count block with one all-reduce (core.process_fastq_sharded); rank 0's output directory is the result.
 
@@ -125,6 +128,13 @@ def bind(CORE=None, engine=None, lib_path=None):
         return reference_around_cut(df_alleles, cut_point, plot_left, plot_right, collapse_by_sequence)
 
     SH.get_dataframe_around_cut_asymmetrical = around_cut
+    # --vcf_output: the edit records built on the GPU, summed natively (vcf.py); the reference's writer formats them
+    from . import vcf
+
+    def build_edit_counts(df_alleles, amplicon_positions):
+        return vcf.build_edit_counts(df_alleles, amplicon_positions, engine=get_engine())
+
+    CORE.vcf.build_edit_counts = build_edit_counts
     return CORE
 
 

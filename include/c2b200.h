@@ -449,6 +449,39 @@ int  c2b_fastq_filter_pair(const char *path1_in, const char *path2_in, const cha
                            int32_t min_bp_qual_in_read, int32_t min_av_read_qual, int32_t min_bp_qual_or_N,
                            int32_t n_threads, int64_t *n_in, int64_t *n_out);
 
+/* ---- --vcf_output edit counts (csrc/c2b_vcf.cuh on the device, the sum in csrc/c2b_fastq.cpp) ----
+ * replaces: build_edit_counts (CRISPResso2/writers/vcf.py:172-212) over the rows of df_alleles that have edits: every deletion,
+ * insertion and substitution of a row becomes one (chrom, pos, REF, ALT) key, deletions and insertions left-normalised
+ * (_left_normalize_deletion / _left_normalize_insertion, :9-40, :79-112), and equal keys sum the rows' #Reads.  The rows come
+ * packed: per row chrom id (< 0: its Reference_Name is not in amplicon_positions), pos (the amplicon's 1-based start), #Reads,
+ * Reference_Sequence / Aligned_Sequence bytes at ref_off / aln_off, ref_positions at rp_off, deletion_coordinates and
+ * insertion_coordinates as (a, b) int64 pairs at del_off / ins_off (offsets counted in pairs), insertion_sizes at isz_off and
+ * substitution_positions at sub_off (every offset array n_rows + 1 long, starting at 0).  Rows go through the device in chunks
+ * of `chunk` rows (<= 0: 16384) through pinned buffers on the engine's stream.
+ * Result: the distinct keys in the order the reference's dict has them (first record in row order, then deletions, insertions,
+ * substitutions), key i at keys[key_off[i] .. key_off[i+1]) as chrom id (int32 LE) | pos (int64 LE) | len(REF) (int32 LE) |
+ * REF | ALT, with its summed #Reads.  When a row raises in the reference, returns C2B_E_ARG with err[0..2] = row, kind
+ * (C2B_VCF_E_*), value (the argument of the failed ref_positions.index() for C2B_VCF_E_NOT_IN_LIST): the first such row, and
+ * in it the first exception in the reference's order.  err[0] = -1 otherwise.  C2B_E_LIMIT: a sum leaves int64.         */
+#define C2B_VCF_E_KEY           1   /* KeyError(Reference_Name) */
+#define C2B_VCF_E_NOT_IN_LIST   2   /* ValueError: <value> is not in list */
+#define C2B_VCF_E_STRING_INDEX  3   /* IndexError: string index out of range */
+#define C2B_VCF_E_EMPTY_MAX     4   /* ValueError: max() iterable argument is empty */
+typedef struct c2b_vcf_counts c2b_vcf_counts;
+int  c2b_vcf_edit_counts(c2b_engine *e, int64_t n_rows, const int32_t *chrom, const int64_t *pos, const int64_t *reads,
+                         const uint8_t *ref, const int64_t *ref_off, const uint8_t *aln, const int64_t *aln_off,
+                         const int64_t *rp, const int64_t *rp_off, const int64_t *del, const int64_t *del_off,
+                         const int64_t *ins, const int64_t *ins_off, const int64_t *isz, const int64_t *isz_off,
+                         const int64_t *sub, const int64_t *sub_off, int64_t chunk, int64_t *err, c2b_vcf_counts **out);
+void c2b_vcf_free(c2b_vcf_counts *v);
+int64_t        c2b_vcf_n(const c2b_vcf_counts *v);             /* distinct keys */
+const uint8_t *c2b_vcf_keys(const c2b_vcf_counts *v);
+const int64_t *c2b_vcf_key_offsets(const c2b_vcf_counts *v);   /* n + 1 */
+const int64_t *c2b_vcf_reads(const c2b_vcf_counts *v);         /* summed #Reads per key */
+int64_t        c2b_vcf_n_records(const c2b_vcf_counts *v);     /* records before the sum */
+/* wall time of the call's device pass with its copies, and of the host sum, in ms */
+int  c2b_vcf_timings(const c2b_vcf_counts *v, double *device_ms, double *sum_ms);
+
 /* ---- paired-end merge mode (csrc/c2b_paired.cpp) ----
  * get_consensus_alignment_from_pairs (CRISPRessoCORE.py:829-985, get_greater_qual_nuc :801-826): the two mates' alignments to one
  * amplicon (aligned read, aligned amplicon, score, quality string of the read's bases) merged column by column into one aligned
