@@ -81,7 +81,8 @@ EDIT_DTYPE = np.dtype([("a", "<u2"), ("b", "<u2"), ("type", "u1"), ("in_window",
 assert ALN_DTYPE.itemsize == 32 and REC_DTYPE.itemsize == 16 and EDIT_DTYPE.itemsize == 8
 
 EXPORTS = ["c2b_create", "c2b_destroy", "c2b_last_error", "c2b_configure", "c2b_set_edit_cap", "c2b_string_width", "c2b_align_batch",
-           "c2b_align_batch_compact", "c2b_ops_words", "c2b_expand_alignment", "c2b_expand_batch", "c2b_ops_device",
+           "c2b_align_batch_compact", "c2b_ops_words", "c2b_expand_alignment", "c2b_expand_batch", "c2b_expand_batch_tables",
+           "c2b_ops_device",
            "c2b_align_batch_device", "c2b_set_pair_order", "c2b_sync", "c2b_stream", "c2b_last_kernel_ms", "c2b_launch_count", "c2b_path_counts", "c2b_band_reruns", "c2b_ring_counts", "c2b_diag_counts", "c2b_route_counts", "c2b_diag_popcount_reads",
            "c2b_counts_layout", "c2b_counts_hist_layout", "c2b_counts_reset", "c2b_counts_read", "c2b_counts_device", "c2b_global_align",
            "c2b_classify_aligned", "c2b_classify_aligned_flags", "c2b_host_alloc", "c2b_host_free",
@@ -136,6 +137,8 @@ def load(path=None):
     L.c2b_expand_alignment.argtypes = [vp, vp, C.c_uint32, C.c_char_p, i32, C.c_char_p, i32, vp, vp]
     L.c2b_expand_batch.restype = C.c_int
     L.c2b_expand_batch.argtypes = [vp, vp, vp, i64, vp, vp, vp, i32, vp, i32]
+    L.c2b_expand_batch_tables.restype = C.c_int
+    L.c2b_expand_batch_tables.argtypes = [vp, vp, i64, vp, vp, vp, i32, i32, i32, C.POINTER(C.c_char_p), vp, vp, vp, i32]
     L.c2b_ops_device.restype = C.c_int
     L.c2b_ops_device.argtypes = [vp, C.POINTER(vp), C.POINTER(vp)]
     L.c2b_align_batch_device.restype = C.c_int

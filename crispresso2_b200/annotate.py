@@ -127,6 +127,8 @@ class Annotation:
         amask, label = np.ascontiguousarray(amask), np.ascontiguousarray(label)
         comp = _comp256()
         eng = src.engine
+        if not eng.h:                                           # the pass runs on the engine's device; its configuration is not read
+            raise core.EngineError("c2b_annotate_build: the engine that ran this batch was closed")
         L = self.L = eng.L
         h = C.c_void_p()
         NW = ops.shape[2]

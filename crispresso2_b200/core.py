@@ -26,8 +26,7 @@ from .resources import payload_from_lists
 
 _COMP = str.maketrans("ACGTN_-", "TGCAN_-")
 _engines = {}
-_blocks = {}
-_sources = {}                     # id(variantCache) -> lazy.BatchSource of the process_fastq call that filled it (alleles.py)
+_empty = {}                       # id(variantCache) -> (weakref to its lazy.BatchSource, the cache): caches a call left empty
 last_timings = {}                 # seconds of the last process_fastq call by stage (bench.py's api leg reports them)
 
 
@@ -497,12 +496,13 @@ def process_fastq(fastq_filename, variantCache, ref_names, refs, args, files_to_
 
 def _result_arrays(res):
     return {"recs": res.recs, "alns": res.alns, "ops": res.ops, "meta": res.meta, "edits": res.edits, "W": res.W,
-            "buf": res._buf, "off": res._off}
+            "buf": res._buf, "off": res._off, "tables": res.tables}
 
 
 def _result_from(engine, d, flags):
     from .engine import BatchResult
-    r = BatchResult(d["recs"], d["alns"], None, d["edits"], d["W"], ops=d["ops"], meta=d["meta"], engine=engine, buf=d["buf"], off=d["off"])
+    r = BatchResult(d["recs"], d["alns"], None, d["edits"], d["W"], ops=d["ops"], meta=d["meta"], lib=engine.L, buf=d["buf"], off=d["off"],
+                    tables=d["tables"])
     r.flags = flags
     return r
 
@@ -656,7 +656,6 @@ def _process_uniques(engine, buf, off, counts, keys, variantCache, ref_names, re
     src = lazy.BatchSource(None, keys_g, ref_names, refs, counts_g, parts=parts)
     src.weights, src.flags, src.lib_path, src.scaffold = weights, flags, engine.lib_path, scaffold
     src.engine, src.packed_all, src.good = engine, (buf, off), (good if n_bad else None)     # annotate.py
-    _sources[id(variantCache)] = src
     cls = src.lazy_class()
     not_aligned = {}
     sel = aligned.astype(np.uint8)
@@ -678,7 +677,8 @@ def _process_uniques(engine, buf, off, counts, keys, variantCache, ref_names, re
             raise EngineError("device aln_stats disagree with per-read records for %s: %d != %d" % (key, val, st[key]))
     for lab, val in extra.items():
         block.class_extra[lab] = block.class_extra.get(lab, 0) + val
-    _blocks[id(variantCache)] = block
+    src.block = block
+    _remember(variantCache, src)
     last_timings["stats_cache"] = time.perf_counter() - t_tab
     return st, not_aligned
 
@@ -716,17 +716,41 @@ def process_fastq_sharded(fastq_filename, variantCache, ref_names, refs, args, f
                             group=world_group)
 
 
+def _remember(variantCache, src):
+    """A cache reaches its call's results through its own entries: every LazyVariant class carries its BatchSource, so the
+    results are released with the cache and its not_aligned_variants dict, and a new dict -- which holds no such entry -- is
+    never answered with the results of a dead cache.  A cache the call left empty (no read aligned) has no entry to go
+    through: it is held here with a weak reference to the results, both dropped when the results die (once the call's
+    not_aligned_variants dict is gone); holding the cache keeps its id from being reused meanwhile."""
+    import weakref
+    src.cache_id = id(variantCache)
+    if variantCache:
+        return
+    key = id(variantCache)
+
+    def gone(ref, key=key):
+        if _empty.get(key, (None,))[0] is ref:
+            del _empty[key]
+    _empty[key] = (weakref.ref(src, gone), variantCache)
+
+
 def source_of(variantCache):
-    """Compact results (lazy.BatchSource) of the process_fastq call that filled this variantCache."""
-    try:
-        return _sources[id(variantCache)]
-    except KeyError:
-        raise KeyError("this variantCache was not filled by crispresso2_b200.core.process_fastq") from None
+    """Compact results (lazy.BatchSource) of the process_fastq call that filled this variantCache.  KeyError for a dict no
+    call filled, and for a cache whose entries have all been popped or replaced by other objects."""
+    for v in variantCache.values():
+        src = getattr(type(v), "_src", None)
+        if src is not None and src.cache_id == id(variantCache):
+            return src
+    held = _empty.get(id(variantCache))
+    src = held[0]() if held is not None and held[1] is variantCache and not variantCache else None
+    if src is None:
+        raise KeyError("this variantCache was not filled by crispresso2_b200.core.process_fastq")
+    return src
 
 
 def quantify(variantCache):
     """Count block accumulated on the device by the process_fastq call that filled this variantCache."""
-    return _blocks[id(variantCache)]
+    return source_of(variantCache).block
 
 
 def get_new_variant_object(args, fastq_seq, refs, ref_names, aln_matrix, pe_scaffold_dna_info=None, engine=None):

@@ -1378,22 +1378,16 @@ int c2b_ops_words(const c2b_engine *e, int32_t max_read_len)
 
 // Aligned strings of one (read, reference) slot from its op stream: host code, no device work.  Column q from the RIGHT
 // end of the alignment is op (ops[q >> 5] >> 2 (q & 31)) & 3: 0 = both consume, 1 = gap in the read, 2 = gap in the
-// reference.  strand 1: the read was aligned as its reverse complement (engine's complement table).
-int c2b_expand_alignment(const c2b_engine *e, const uint64_t *ops, uint32_t meta, const char *read, int32_t read_len,
-                         const char *ref, int32_t ref_len, char *out_read, char *out_ref)
+// reference.  strand 1: the read was aligned as its reverse complement (comp256: the complement of every byte).
+static int expand_slot(const uint8_t *comp256, const uint64_t *ops, uint32_t meta, const char *read, int32_t read_len,
+                       const char *ref, int32_t ref_len, char *out_read, char *out_ref)
 {
-    if (!e || !ops || !read || !ref || !out_read || !out_ref) return C2B_E_ARG;
     const int n = (int)(meta & 0xffffu), strand = (int)((meta >> 16) & 1u);
-    unsigned char comp[256];
-    if (strand) {
-        for (int c = 0; c < 256; c++) comp[c] = (unsigned char)c;
-        for (int q = 0; q < e->prm.nq; q++) comp[(unsigned char)e->prm.alphabet[q]] = (unsigned char)e->prm.alphabet[e->prm.complement[q]];
-    }
     int i = ref_len, j = read_len;
     for (int q = 0; q < n; q++) {
         const int op = (int)((ops[q >> 5] >> (2 * (q & 31))) & 3ull);
         char rd = '-', rf = '-';
-        if (op != OP_J) { if (j < 1) return C2B_E_ARG; j--; rd = strand ? (char)comp[(unsigned char)read[read_len - 1 - j]] : read[j]; }
+        if (op != OP_J) { if (j < 1) return C2B_E_ARG; j--; rd = strand ? (char)comp256[(unsigned char)read[read_len - 1 - j]] : read[j]; }
         if (op != OP_I) { if (i < 1) return C2B_E_ARG; i--; rf = ref[i]; }
         if (op == OP_NONE) return C2B_E_ARG;
         out_read[n - 1 - q] = rd; out_ref[n - 1 - q] = rf;
@@ -1401,28 +1395,50 @@ int c2b_expand_alignment(const c2b_engine *e, const uint64_t *ops, uint32_t meta
     return (i == 0 && j == 0) ? C2B_OK : C2B_E_ARG;
 }
 
-// Batch form: strings[n_reads][R][2][W], right-aligned like c2b_align_batch's, from the compact outputs; host threads.
-int c2b_expand_batch(const c2b_engine *e, const uint8_t *reads, const int64_t *offsets, int64_t n_reads, const int32_t *ref_id,
-                     const uint64_t *ops, const uint32_t *meta, int32_t max_read_len, uint8_t *strings, int32_t n_threads)
+// the engine's complement table (c2b_params.complement) over all bytes, identity outside the alphabet
+static void engine_comp256(const c2b_engine *e, uint8_t *comp)
 {
-    if (!e || !e->configured || !reads || !offsets || !ops || !meta || !strings) return C2B_E_ARG;
-    const int W = (e->max_I + max_read_len + 31) & ~31, NW = W / 32, nr = ref_id ? 1 : e->n_refs;
+    for (int c = 0; c < 256; c++) comp[c] = (uint8_t)c;
+    for (int q = 0; q < e->prm.nq; q++) comp[(unsigned char)e->prm.alphabet[q]] = (uint8_t)e->prm.alphabet[e->prm.complement[q]];
+}
+
+int c2b_expand_alignment(const c2b_engine *e, const uint64_t *ops, uint32_t meta, const char *read, int32_t read_len,
+                         const char *ref, int32_t ref_len, char *out_read, char *out_ref)
+{
+    if (!e || !ops || !read || !ref || !out_read || !out_ref) return C2B_E_ARG;
+    uint8_t comp[256];
+    engine_comp256(e, comp);
+    return expand_slot(comp, ops, meta, read, read_len, ref, ref_len, out_read, out_ref);
+}
+
+// Batch form over explicit tables: strings[n_reads][R][2][W], right-aligned like c2b_align_batch's; host threads.  Nothing is
+// read from an engine, so a batch's results spell the same strings whatever their engine was configured with since.
+int c2b_expand_batch_tables(const uint8_t *reads, const int64_t *offsets, int64_t n_reads, const int32_t *ref_id,
+                            const uint64_t *ops, const uint32_t *meta, int32_t R, int32_t W, int32_t n_refs,
+                            const char *const *ref_seqs, const int32_t *ref_lens, const uint8_t *comp256,
+                            uint8_t *strings, int32_t n_threads)
+{
+    if (n_reads < 0 || (n_reads && (!reads || !offsets || !ops || !meta || !strings)) || !ref_seqs || !ref_lens || !comp256)
+        return C2B_E_ARG;
+    if (W < 32 || (W & 31) || n_refs < 1 || R < 1 || (ref_id ? R != 1 : R > n_refs)) return C2B_E_ARG;
+    for (int r = 0; r < n_refs; r++) if (!ref_seqs[r] || ref_lens[r] < 1) return C2B_E_ARG;
+    const int NW = W / 32;
     if (n_threads <= 0) n_threads = (int)std::max(1u, std::thread::hardware_concurrency());
     n_threads = (int)std::min<int64_t>(n_threads, std::max<int64_t>(1, n_reads / 1024));
     std::vector<int> bad((size_t)n_threads, 0);
     auto work = [&](int t) {
         const int64_t lo = n_reads * t / n_threads, hi = n_reads * (t + 1) / n_threads;
         for (int64_t rd = lo; rd < hi; rd++)
-            for (int k = 0; k < nr; k++) {
+            for (int k = 0; k < R; k++) {
                 const int r = ref_id ? ref_id[rd] : k;
-                const int64_t slot = rd * nr + k;
+                const int64_t slot = rd * R + k;
                 const uint32_t m = meta[slot];
                 const int n = (int)(m & 0xffffu);
                 if ((m >> 24) == 0 || n == 0 || n > W) continue;      // no alignment in this slot
+                if (r < 0 || r >= n_refs) { bad[(size_t)t]++; continue; }
                 uint8_t *o = strings + slot * 2 * (int64_t)W;
-                const RefHost &R = e->refs[(size_t)r];
-                if (c2b_expand_alignment(e, ops + slot * NW, m, (const char *)reads + offsets[rd], (int32_t)(offsets[rd + 1] - offsets[rd]),
-                                         R.seq.data(), (int32_t)R.seq.size(), (char *)o + W - n, (char *)o + 2 * W - n)) bad[(size_t)t]++;
+                if (expand_slot(comp256, ops + slot * NW, m, (const char *)reads + offsets[rd], (int32_t)(offsets[rd + 1] - offsets[rd]),
+                                ref_seqs[r], ref_lens[r], (char *)o + W - n, (char *)o + 2 * W - n)) bad[(size_t)t]++;
             }
     };
     std::vector<std::thread> th;
@@ -1431,6 +1447,21 @@ int c2b_expand_batch(const c2b_engine *e, const uint8_t *reads, const int64_t *o
     for (auto &x : th) x.join();
     for (int b : bad) if (b) return C2B_E_ARG;
     return C2B_OK;
+}
+
+// Batch form over the engine's current configuration (the batch must have run under it)
+int c2b_expand_batch(const c2b_engine *e, const uint8_t *reads, const int64_t *offsets, int64_t n_reads, const int32_t *ref_id,
+                     const uint64_t *ops, const uint32_t *meta, int32_t max_read_len, uint8_t *strings, int32_t n_threads)
+{
+    if (!e || !e->configured || !reads || !offsets || !ops || !meta || !strings) return C2B_E_ARG;
+    const int W = (e->max_I + max_read_len + 31) & ~31, nr = ref_id ? 1 : e->n_refs;
+    std::vector<const char *> seqs((size_t)e->n_refs);
+    std::vector<int32_t> lens((size_t)e->n_refs);
+    for (int r = 0; r < e->n_refs; r++) { seqs[(size_t)r] = e->refs[(size_t)r].seq.data(); lens[(size_t)r] = (int32_t)e->refs[(size_t)r].seq.size(); }
+    uint8_t comp[256];
+    engine_comp256(e, comp);
+    return c2b_expand_batch_tables(reads, offsets, n_reads, ref_id, ops, meta, nr, W, e->n_refs, seqs.data(), lens.data(), comp,
+                                   strings, n_threads);
 }
 
 int c2b_counts_layout(const c2b_engine *e, int32_t *n_refs, int32_t *n_vec, int32_t *stride, int32_t *n_scal)

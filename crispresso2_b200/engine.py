@@ -26,26 +26,37 @@ class BatchResult:
     edits   : EDIT_DTYPE [n, R, cap] or None
     ops/meta: compact form (c2b_align_batch_compact): uint64 [n, R, W/32] op streams, uint32 [n, R] meta words; the strings
               of any block of reads are rebuilt on demand by the library's host-side expansion (strings_block)
+    A compact result owns what its expansion needs -- the configured reference sequences, the string width and the complement
+    table the batch ran with (`tables`, Engine.tables) -- so it spells the same strings whatever its engine does afterwards:
+    reconfigured for another run, used for a batch of another size, or closed.
     """
 
-    def __init__(self, recs, alns, strings, edits, W, ops=None, meta=None, engine=None, buf=None, off=None, ref_id=None):
+    def __init__(self, recs, alns, strings, edits, W, ops=None, meta=None, lib=None, buf=None, off=None, ref_id=None, tables=None):
         self.recs, self.alns, self.strings, self.edits, self.W = recs, alns, strings, edits, W
-        self.ops, self.meta, self._engine, self._buf, self._off, self._ref_id = ops, meta, engine, buf, off, ref_id
+        self.ops, self.meta, self._lib, self._buf, self._off, self._ref_id = ops, meta, lib, buf, off, ref_id
+        self.tables = tables
+        if ops is not None:
+            seqs, comp = tables
+            self._c_seqs = (C.c_char_p * len(seqs))(*seqs)
+            self._c_lens = np.asarray([len(x) for x in seqs], dtype=np.int32)
+            self._c_comp = np.ascontiguousarray(comp, dtype=np.uint8)
 
     def strings_block(self, lo, hi):
         """uint8 [hi-lo, R, 2, W] aligned strings of reads lo..hi-1"""
         if self.strings is not None:
             return self.strings[lo:hi]
-        e = self._engine
         off = np.ascontiguousarray(self._off[lo:hi + 1])
         rid = None if self._ref_id is None else np.ascontiguousarray(self._ref_id[lo:hi], dtype=np.int32)
         ops = np.ascontiguousarray(self.ops[lo:hi])
         meta = np.ascontiguousarray(self.meta[lo:hi])
-        out = np.zeros((hi - lo, self.alns.shape[1], 2, self.W), dtype=np.uint8)
-        maxj = e._max_len_of(self.W)
-        e._check(e.L.c2b_expand_batch(e.h, self._buf.ctypes.data, off.ctypes.data, hi - lo,
-                                      rid.ctypes.data if rid is not None else None, ops.ctypes.data, meta.ctypes.data,
-                                      maxj, out.ctypes.data, 0), "c2b_expand_batch")
+        R = self.alns.shape[1]
+        out = np.zeros((hi - lo, R, 2, self.W), dtype=np.uint8)
+        rc = self._lib.c2b_expand_batch_tables(self._buf.ctypes.data, off.ctypes.data, hi - lo,
+                                               rid.ctypes.data if rid is not None else None, ops.ctypes.data, meta.ctypes.data,
+                                               R, self.W, len(self._c_lens), self._c_seqs, self._c_lens.ctypes.data,
+                                               self._c_comp.ctypes.data, out.ctypes.data, 0)
+        if rc != 0:
+            raise EngineError("c2b_expand_batch_tables failed (%d): an op stream does not fit its read and reference" % rc)
         return out
 
     def pair(self, i, r=0):
@@ -83,6 +94,7 @@ class Engine:
         self.alphabet = "ACGTN"
         self.edit_cap = 0
         self._keep = None
+        self.tables = None
 
     def close(self):
         if getattr(self, "h", None):
@@ -153,6 +165,10 @@ class Engine:
         self.ref_lens = [len(refs[n]["sequence"]) for n in ref_names]
         self.ref_seqs = [refs[n]["sequence"] for n in ref_names]
         self.flags = int(flags)
+        comp = np.arange(256, dtype=np.uint8)              # p.complement over every byte, identity outside the alphabet
+        for q, ch in enumerate(alphabet):
+            comp[ord(ch)] = ord(alphabet[p.complement[q]])
+        self.tables = (tuple(k[0] for k in keep), comp)    # what a compact BatchResult needs to spell its strings
         return self
 
     def set_edit_cap(self, cap):
@@ -165,10 +181,6 @@ class Engine:
         if w < 0:
             raise EngineError("engine not configured")
         return w
-
-    def _max_len_of(self, W):
-        """a max_read_len that reproduces string width W (c2b_string_width rounds max_I + max_read_len up to 32)"""
-        return max(1, W - max(self.ref_lens))
 
     def align_packed(self, buf, off, count=None, qweight=None, ref_id=None, strings=True, edits=True, compact=False, on_launch=None):
         """One batch through the host-buffer entry.  compact=True: op streams + meta words come back instead of the aligned
@@ -197,7 +209,8 @@ class Engine:
             self._check(self.L.c2b_align_batch_compact(self.h, ptr(buf) if len(buf) else None, ptr(off), n, ptr(cnt), ptr(qw),
                                                        ptr(rid), ptr(recs), ptr(alns), ptr(ops), ptr(meta), ptr(earr)),
                         "c2b_align_batch_compact")
-            return BatchResult(recs, alns, None, earr, W, ops=ops, meta=meta, engine=self, buf=buf, off=off, ref_id=rid)
+            return BatchResult(recs, alns, None, earr, W, ops=ops, meta=meta, lib=self.L, buf=buf, off=off, ref_id=rid,
+                               tables=self.tables)
         sarr = np.zeros((n, nr, 2, W), dtype=np.uint8) if strings else None
         self._check(self.L.c2b_align_batch(self.h, ptr(buf) if len(buf) else None, ptr(off), n, ptr(cnt), ptr(qw),
                                            ptr(rid), ptr(recs), ptr(alns), ptr(sarr), ptr(earr)), "c2b_align_batch")

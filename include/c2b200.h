@@ -229,9 +229,20 @@ int  c2b_ops_words(const c2b_engine *e, int32_t max_read_len);
 /* out_read / out_ref receive (meta & 0xffff) characters each, left to right as global_align returns them (Align.pyx:422-434) */
 int  c2b_expand_alignment(const c2b_engine *e, const uint64_t *ops, uint32_t meta, const char *read, int32_t read_len,
                           const char *ref, int32_t ref_len, char *out_read, char *out_ref);
-/* strings: n_reads * R * 2 * W bytes, right-aligned slots as c2b_align_batch writes them; host threads (n_threads <= 0: all) */
+/* strings: n_reads * R * 2 * W bytes, right-aligned slots as c2b_align_batch writes them; host threads (n_threads <= 0: all).
+ * Reads the engine's CURRENT references, max_I and complement table: valid only while the engine keeps the configuration the
+ * batch ran under. */
 int  c2b_expand_batch(const c2b_engine *e, const uint8_t *reads, const int64_t *offsets, int64_t n_reads, const int32_t *ref_id,
                       const uint64_t *ops, const uint32_t *meta, int32_t max_read_len, uint8_t *strings, int32_t n_threads);
+/* Same, with no engine: the caller passes what the batch ran with -- R slots per read (1 with ref_id), the string width W
+ * (a multiple of 32; NW = W / 32 op words per slot), the n_refs configured reference sequences and their lengths, and the
+ * complement of every byte (identity outside the alphabet).  A batch's results expand the same way whatever its engine does
+ * afterwards, closed included.  C2B_E_ARG on an op stream that does not fit its read and reference, or a ref_id outside
+ * 0..n_refs-1. */
+int  c2b_expand_batch_tables(const uint8_t *reads, const int64_t *offsets, int64_t n_reads, const int32_t *ref_id,
+                             const uint64_t *ops, const uint32_t *meta, int32_t R, int32_t W, int32_t n_refs,
+                             const char *const *ref_seqs, const int32_t *ref_lens, const uint8_t *comp256,
+                             uint8_t *strings, int32_t n_threads);
 
 /* Same, with every pointer a DEVICE pointer on the engine's device and no copies; the launch is queued on
  * the engine's stream.  max_read_len must bound the reads.  Use c2b_sync() before reading results.     */
