@@ -36,6 +36,8 @@ ST_EDIT_OVERFLOW = 4
 E_ARG, E_LIMIT, E_STATE = -2, -3, -4                    # C2B_E_* of include/c2b200.h
 ST_TOO_LONG = 8
 VCF_E_KEY, VCF_E_NOT_IN_LIST, VCF_E_STRING_INDEX, VCF_E_EMPTY_MAX = 1, 2, 3, 4     # C2B_VCF_E_*: c2b_vcf_edit_counts' err[1]
+BE_E_STRING_INDEX = 1                                   # C2B_BE_E_*: c2b_be_upset_counts' err[1]
+BE_N_TOTALS = 10                                        # C2B_BE_N_TOTALS
 
 # count-block layout (enum order of c2b200.h)
 V_ALL_INS, V_ALL_INS_LEFT, V_ALL_DEL, V_ALL_SUB, V_INS, V_DEL, V_SUB, V_SUBBASE0 = range(8)
@@ -95,7 +97,10 @@ EXPORTS = ["c2b_create", "c2b_destroy", "c2b_last_error", "c2b_configure", "c2b_
            "c2b_annotate_cigar_arena", "c2b_annotate_cigar_offsets", "c2b_annotate_flags", "c2b_annotate_mapq", "c2b_annotate_first",
            "c2b_annotate_last_record", "c2b_annotate_record_arena", "c2b_annotate_record_offsets", "c2b_annotate_write_fastq",
            "c2b_annotate_write_sam", "c2b_annotate_write_sam_passthrough", "c2b_vcf_edit_counts", "c2b_vcf_free", "c2b_vcf_n",
-           "c2b_vcf_keys", "c2b_vcf_key_offsets", "c2b_vcf_reads", "c2b_vcf_n_records", "c2b_vcf_timings"]
+           "c2b_vcf_keys", "c2b_vcf_key_offsets", "c2b_vcf_reads", "c2b_vcf_n_records", "c2b_vcf_timings",
+           "c2b_be_upset_counts", "c2b_be_upset_free", "c2b_be_upset_n", "c2b_be_upset_keys", "c2b_be_upset_key_offsets",
+           "c2b_be_upset_reads", "c2b_be_upset_totals", "c2b_be_upset_timings", "c2b_be_quilt_table", "c2b_be_quilt_free",
+           "c2b_be_quilt_n", "c2b_be_quilt_bytes", "c2b_be_quilt_fetch", "c2b_be_quilt_timings"]
 
 _cache = {}
 
@@ -271,5 +276,19 @@ def load(path=None):
         getattr(L, name).argtypes = [vp]
     L.c2b_vcf_timings.restype = C.c_int
     L.c2b_vcf_timings.argtypes = [vp, C.POINTER(C.c_double), C.POINTER(C.c_double)]
+    L.c2b_be_upset_counts.restype = C.c_int
+    L.c2b_be_upset_counts.argtypes = [vp, i64] + [vp] * 6 + [i32] + [vp] * 3 + [i64, vp, C.POINTER(vp)]
+    L.c2b_be_quilt_table.restype = C.c_int
+    L.c2b_be_quilt_table.argtypes = [vp, i64, i32] + [vp] * 10 + [i64, vp, C.POINTER(vp)]
+    for name, rt in (("c2b_be_upset_free", None), ("c2b_be_upset_n", i64), ("c2b_be_upset_keys", vp), ("c2b_be_upset_key_offsets", vp),
+                     ("c2b_be_upset_reads", vp), ("c2b_be_upset_totals", vp), ("c2b_be_quilt_free", None), ("c2b_be_quilt_n", i64),
+                     ("c2b_be_quilt_bytes", i64)):
+        getattr(L, name).restype = rt
+        getattr(L, name).argtypes = [vp]
+    L.c2b_be_quilt_fetch.restype = C.c_int
+    L.c2b_be_quilt_fetch.argtypes = [vp] * 9
+    for name in ("c2b_be_upset_timings", "c2b_be_quilt_timings"):
+        getattr(L, name).restype = C.c_int
+        getattr(L, name).argtypes = [vp, C.POINTER(C.c_double), C.POINTER(C.c_double)]
     _cache[path] = L
     return L

@@ -7,7 +7,8 @@
 //   * CRISPRessoShared.get_dataframe_around_cut_asymmetrical / get_dataframe_around_cut (CRISPRessoShared.py:1513-1531):
 //     per allele the window [cut_idx - left + 1, cut_idx + right + 1) of both aligned strings (cut_idx = the column that holds
 //     reference position cut_point, i.e. row['ref_positions'].index(cut_point)), pandas groupby(...).sum() over the six key
-//     columns and the final sort.
+//     columns and the final sort -- the grouping, with its Kahan sum and sort, shared with the --base_editor_output quilt table
+//     (c2b_group_around_cut, called by c2b_be_quilt_table in c2b_engine.cu).
 // Nothing here aligns or classifies: rows arrive with their alignment (ops) and their per-read numbers (n_deleted, ...,
 // Read_Status) as the GPU produced them; this file spells strings, sorts, groups and formats -- the work pandas does row by
 // row in the reference (10 % of a reference run's time, SURVEY.md section 8f rank 2).
@@ -25,17 +26,11 @@
 #include <vector>
 
 #include "c2b200.h"
+#include "c2b_fastq_int.h"
 
 namespace {
 
 constexpr int OP_M = 0, OP_J = 1, OP_I = 2, OP_NONE = 3;
-
-struct Group {
-    int64_t first_row;        // a row that carries the window strings
-    int32_t s0, s1;           // window [s0, s1) of that row's columns
-    uint8_t unedited; int32_t ndel, nins, nmut;
-    int64_t reads; double pct, comp;
-};
 
 }  // namespace
 
@@ -47,7 +42,7 @@ struct c2b_alleles {
     std::vector<int64_t> count;
     std::vector<int64_t> order;            // rows sorted by (#Reads desc, Aligned_Sequence, Reference_Sequence), stable
     // result of the last c2b_alleles_around_cut
-    std::vector<Group> groups;
+    std::vector<c2b_cut_group> groups;       // window strings point into arena
     int32_t win_max = 0;
     std::string err;
 };
@@ -205,6 +200,8 @@ int c2b_alleles_write_tsv(const c2b_alleles *A, const char *path, int64_t n_sel,
     return ok ? C2B_OK : C2B_E_ARG;
 }
 
+}  // extern "C"
+
 // pandas' group_sum for float64 (Kahan): one addend
 static inline void group_add(double &sumx, double &comp, double val)
 {
@@ -214,6 +211,59 @@ static inline void group_add(double &sumx, double &comp, double val)
     if (comp != comp) comp = 0;                             // inf - inf
     sumx = t;
 }
+
+// pandas' groupby(six key columns).sum() over `rows` in row order (#Reads in int64, %Reads with group_add), then
+// sort_values(['#Reads', 'Aligned_Sequence', 'Reference_Sequence'], ascending=[False, True, True]) from groupby's key order
+std::vector<c2b_cut_group> c2b_group_around_cut(const std::vector<c2b_cut_group> &rows)
+{
+    std::vector<c2b_cut_group> groups;
+    std::unordered_multimap<uint64_t, int64_t> index;
+    index.reserve(std::min<size_t>(rows.size(), (size_t)1 << 20));
+    for (const c2b_cut_group &R : rows) {
+        uint64_t h = 1469598103934665603ull;
+        auto mix = [&](uint64_t v) { h ^= v; h *= 1099511628211ull; };
+        for (int64_t x = 0; x < R.len; x++) mix(R.seq[x]);
+        mix(0x100);
+        for (int64_t x = 0; x < R.len; x++) mix(R.ref[x]);
+        mix(R.unedited ? 0x201 : 0x200); mix((uint64_t)R.ndel); mix((uint64_t)R.nins + 0x1000000ull); mix((uint64_t)R.nmut + 0x2000000ull);
+        int64_t g = -1;
+        auto range = index.equal_range(h);
+        for (auto it = range.first; it != range.second; ++it) {
+            const c2b_cut_group &G = groups[(size_t)it->second];
+            if (G.len != R.len || G.unedited != R.unedited || G.ndel != R.ndel || G.nins != R.nins || G.nmut != R.nmut) continue;
+            if (memcmp(G.seq, R.seq, (size_t)R.len) || memcmp(G.ref, R.ref, (size_t)R.len)) continue;
+            g = it->second; break;
+        }
+        if (g < 0) {
+            c2b_cut_group G = R;
+            G.reads = 0; G.pct = 0.0; G.comp = 0.0;
+            g = (int64_t)groups.size();
+            groups.push_back(G);
+            index.emplace(h, g);
+        }
+        c2b_cut_group &G = groups[(size_t)g];
+        G.reads += R.reads;
+        group_add(G.pct, G.comp, R.pct);
+    }
+    // groupby order (keys ascending) refined by the final sort_values(#Reads desc, Aligned_Sequence, Reference_Sequence), stable
+    auto scmp = [](const uint8_t *pa, int64_t la, const uint8_t *pb, int64_t lb) {
+        const int c = memcmp(pa, pb, (size_t)std::min(la, lb));
+        if (c) return c;
+        return la < lb ? -1 : la > lb ? 1 : 0;
+    };
+    std::sort(groups.begin(), groups.end(), [&](const c2b_cut_group &a, const c2b_cut_group &b) {
+        if (a.reads != b.reads) return a.reads > b.reads;
+        int c = scmp(a.seq, a.len, b.seq, b.len); if (c) return c < 0;
+        c = scmp(a.ref, a.len, b.ref, b.len); if (c) return c < 0;
+        if (a.unedited != b.unedited) return a.unedited < b.unedited;
+        if (a.ndel != b.ndel) return a.ndel < b.ndel;
+        if (a.nins != b.nins) return a.nins < b.nins;
+        return a.nmut < b.nmut;
+    });
+    return groups;
+}
+
+extern "C" {
 
 // get_dataframe_around_cut_asymmetrical over the rows `rows` (in the DataFrame's row order).  Returns the number of groups
 // (< 0: error); fetch them with c2b_alleles_cut_fetch.  C2B_E_LIMIT: some row's alignment does not hold reference position
@@ -225,9 +275,6 @@ int64_t c2b_alleles_around_cut(c2b_alleles *A, int64_t n_sel, const int64_t *row
     if (!A || n_sel < 0 || (n_sel && (!rows || !unedited || !n_deleted || !n_inserted || !n_mutated || !pct)) || cut_point < 0) return C2B_E_ARG;
     A->groups.clear();
     A->win_max = 0;
-    struct Key { uint64_t h; int64_t g; };
-    std::unordered_multimap<uint64_t, int64_t> index;
-    index.reserve((size_t)std::min<int64_t>(n_sel, 1 << 20));
     auto window_of = [&](int64_t r, int &s0, int &s1) -> bool {
         const int n = A->len[(size_t)r];
         const uint8_t *rf = A->arena.data() + A->off[(size_t)r] + n;
@@ -243,60 +290,20 @@ int64_t c2b_alleles_around_cut(c2b_alleles *A, int64_t n_sel, const int64_t *row
         s0 = (int)a; s1 = (int)b;
         return true;
     };
+    std::vector<c2b_cut_group> cut((size_t)n_sel);
     for (int64_t k = 0; k < n_sel; k++) {
         const int64_t r = rows[k];
         if (r < 0 || r >= A->n) return C2B_E_ARG;
         int s0, s1;
         if (!window_of(r, s0, s1)) return C2B_E_LIMIT;
-        const int n = A->len[(size_t)r], wl = s1 - s0;
         const uint8_t *p = A->arena.data() + A->off[(size_t)r];
-        uint64_t h = 1469598103934665603ull;
-        auto mix = [&](uint64_t v) { h ^= v; h *= 1099511628211ull; };
-        for (int x = 0; x < wl; x++) mix(p[s0 + x]);
-        mix(0x100);
-        for (int x = 0; x < wl; x++) mix(p[n + s0 + x]);
-        mix(unedited[r] ? 0x201 : 0x200); mix((uint64_t)(uint32_t)n_deleted[r]); mix((uint64_t)(uint32_t)n_inserted[r] + 0x1000000ull);
-        mix((uint64_t)(uint32_t)n_mutated[r] + 0x2000000ull);
-        int64_t g = -1;
-        auto range = index.equal_range(h);
-        for (auto it = range.first; it != range.second; ++it) {
-            const Group &G = A->groups[(size_t)it->second];
-            if (G.s1 - G.s0 != wl || G.unedited != (unedited[r] ? 1 : 0) || G.ndel != n_deleted[r] || G.nins != n_inserted[r] || G.nmut != n_mutated[r]) continue;
-            const int gn = A->len[(size_t)G.first_row];
-            const uint8_t *gp = A->arena.data() + A->off[(size_t)G.first_row];
-            if (memcmp(gp + G.s0, p + s0, (size_t)wl) || memcmp(gp + gn + G.s0, p + n + s0, (size_t)wl)) continue;
-            g = it->second; break;
-        }
-        if (g < 0) {
-            Group G; G.first_row = r; G.s0 = s0; G.s1 = s1; G.unedited = unedited[r] ? 1 : 0; G.ndel = n_deleted[r]; G.nins = n_inserted[r];
-            G.nmut = n_mutated[r]; G.reads = 0; G.pct = 0.0; G.comp = 0.0;
-            g = (int64_t)A->groups.size();
-            A->groups.push_back(G);
-            index.emplace(h, g);
-            if (wl > A->win_max) A->win_max = wl;
-        }
-        Group &G = A->groups[(size_t)g];
-        G.reads += A->count[(size_t)r];
-        group_add(G.pct, G.comp, pct[r]);
+        c2b_cut_group &G = cut[(size_t)k];
+        G.seq = p + s0; G.ref = p + A->len[(size_t)r] + s0; G.len = s1 - s0;
+        G.unedited = unedited[r] ? 1 : 0; G.ndel = n_deleted[r]; G.nins = n_inserted[r]; G.nmut = n_mutated[r];
+        G.reads = A->count[(size_t)r]; G.pct = pct[r];
     }
-    // groupby order (keys ascending) refined by the final sort_values(#Reads desc, Aligned_Sequence, Reference_Sequence), stable
-    auto wcmp = [&](const Group &a, const Group &b, int part) {
-        const int la = a.s1 - a.s0, lb = b.s1 - b.s0;
-        const uint8_t *pa = A->arena.data() + A->off[(size_t)a.first_row] + (part ? A->len[(size_t)a.first_row] : 0) + a.s0;
-        const uint8_t *pb = A->arena.data() + A->off[(size_t)b.first_row] + (part ? A->len[(size_t)b.first_row] : 0) + b.s0;
-        const int c = memcmp(pa, pb, (size_t)std::min(la, lb));
-        if (c) return c;
-        return la < lb ? -1 : la > lb ? 1 : 0;
-    };
-    std::sort(A->groups.begin(), A->groups.end(), [&](const Group &a, const Group &b) {
-        if (a.reads != b.reads) return a.reads > b.reads;
-        int c = wcmp(a, b, 0); if (c) return c < 0;
-        c = wcmp(a, b, 1); if (c) return c < 0;
-        if (a.unedited != b.unedited) return a.unedited < b.unedited;
-        if (a.ndel != b.ndel) return a.ndel < b.ndel;
-        if (a.nins != b.nins) return a.nins < b.nins;
-        return a.nmut < b.nmut;
-    });
+    A->groups = c2b_group_around_cut(cut);
+    for (const c2b_cut_group &G : A->groups) if (G.len > A->win_max) A->win_max = (int32_t)G.len;
     return (int64_t)A->groups.size();
 }
 
@@ -309,13 +316,11 @@ int c2b_alleles_cut_fetch(const c2b_alleles *A, uint8_t *seq, uint8_t *ref, int3
     if (!A || !seq || !ref || !wlen || !unedited || !n_deleted || !n_inserted || !n_mutated || !reads || !pct) return C2B_E_ARG;
     const int W = A->win_max;
     for (size_t g = 0; g < A->groups.size(); g++) {
-        const Group &G = A->groups[g];
-        const int n = A->len[(size_t)G.first_row], wl = G.s1 - G.s0;
-        const uint8_t *p = A->arena.data() + A->off[(size_t)G.first_row];
-        memcpy(seq + g * (size_t)W, p + G.s0, (size_t)wl);
-        memcpy(ref + g * (size_t)W, p + n + G.s0, (size_t)wl);
-        wlen[g] = wl; unedited[g] = G.unedited; n_deleted[g] = G.ndel; n_inserted[g] = G.nins; n_mutated[g] = G.nmut;
-        reads[g] = G.reads; pct[g] = G.pct;
+        const c2b_cut_group &G = A->groups[g];
+        memcpy(seq + g * (size_t)W, G.seq, (size_t)G.len);
+        memcpy(ref + g * (size_t)W, G.ref, (size_t)G.len);
+        wlen[g] = (int32_t)G.len; unedited[g] = G.unedited; n_deleted[g] = (int32_t)G.ndel; n_inserted[g] = (int32_t)G.nins;
+        n_mutated[g] = (int32_t)G.nmut; reads[g] = G.reads; pct[g] = G.pct;
     }
     return C2B_OK;
 }

@@ -25,6 +25,7 @@
 #include "c2b_split.cuh"
 #include "c2b_annotate.cuh"
 #include "c2b_vcf.cuh"
+#include "c2b_base_edit.cuh"
 #include "c2b_fastq_int.h"
 
 using namespace c2b;
@@ -1762,9 +1763,161 @@ const int64_t *c2b_annotate_last_record(const c2b_annotation *a) { return a && !
 const uint8_t *c2b_annotate_record_arena(const c2b_annotation *a) { return a ? (const uint8_t *)a->rec.data() : nullptr; }
 const int64_t *c2b_annotate_record_offsets(const c2b_annotation *a) { return a && !a->rec_off.empty() ? a->rec_off.data() : nullptr; }
 
-// --vcf_output edit counts (c2b_vcf.cuh) for packed allele rows in chunks: the chunk's rows go up through one pinned buffer, a
-// size pass notes every row's records, bytes and first exception, a scan places them, a write pass builds the records, which
-// come back through a second pinned buffer.  The records of all chunks are then summed on the host (c2b_vcf_sum_records).
+}  // extern "C"
+
+// ----------------------------------------------------------------------------------------- packed allele rows in chunks
+// --vcf_output and --base_editor_output pass allele rows to the device as packed columns, a chunk of rows at a time: the
+// chunk's columns go up through one pinned buffer, per-row sizes and scans live in a second device buffer, results come back
+// through a second pinned buffer.
+
+// one packed column: `width` bytes per row (off == nullptr), or per row the items [off[r], off[r+1]) of `width` bytes each
+struct RowCol { const void *val; const int64_t *off; size_t width; };
+
+struct ChunkPipe {
+    c2b_engine *e;
+    DevBuf d_in, d_len, d_out, d_fixed;
+    uint8_t *h_in = nullptr, *h_out = nullptr; size_t h_in_cap = 0, h_out_cap = 0;
+    explicit ChunkPipe(c2b_engine *e_) : e(e_) {}
+    ~ChunkPipe() { rt_free(d_in.p); rt_free(d_len.p); rt_free(d_out.p); rt_free(d_fixed.p); rt_host_free(h_in); rt_host_free(h_out); }
+    static size_t al(size_t x) { return (x + 255) & ~(size_t)255; }
+    static bool grow(uint8_t *&p, size_t &cap, size_t n)
+    {
+        if (n <= cap) return true;
+        rt_host_free(p); cap = n + n / 4 + 4096; p = (uint8_t *)rt_host_alloc(cap);
+        return p != nullptr;
+    }
+    // rows [r0, r1) of the columns to the device: dev[c] their values, doff[c] their offsets rebased to the chunk (ragged columns)
+    int upload(const RowCol *cols, int nc, int64_t r0, int64_t r1, const char **dev, const int64_t **doff)
+    {
+        const int64_t m = r1 - r0;
+        std::vector<size_t> o_val((size_t)nc), o_off((size_t)nc);
+        size_t o = 0;
+        for (int c = 0; c < nc; c++) {
+            o_val[(size_t)c] = o;
+            o += al(cols[c].off ? (size_t)(cols[c].off[r1] - cols[c].off[r0]) * cols[c].width : (size_t)m * cols[c].width);
+            o_off[(size_t)c] = o;
+            if (cols[c].off) o += al((size_t)(m + 1) * 8);
+        }
+        if (!grow(h_in, h_in_cap, o)) return fail(e, C2B_E_CUDA, "packed rows: pinned allocation");
+        for (int c = 0; c < nc; c++) {
+            const RowCol &k = cols[c];
+            const int64_t b = k.off ? k.off[r0] : r0;
+            const size_t nb = (size_t)((k.off ? k.off[r1] : r1) - b) * k.width;
+            if (nb) memcpy(h_in + o_val[(size_t)c], (const uint8_t *)k.val + (size_t)b * k.width, nb);
+            if (k.off) {
+                int64_t *ho = (int64_t *)(h_in + o_off[(size_t)c]);
+                for (int64_t r = 0; r <= m; r++) ho[r] = k.off[r0 + r] - b;
+            }
+        }
+        int rc;
+        if ((rc = ensure(e, d_in, o))) return rc;
+        RTCHK(rt_h2d(d_in.p, h_in, o, e->stream));
+        for (int c = 0; c < nc; c++) {
+            dev[c] = (const char *)d_in.p + o_val[(size_t)c];
+            if (doff) doff[c] = cols[c].off ? (const int64_t *)((const char *)d_in.p + o_off[(size_t)c]) : nullptr;
+        }
+        return C2B_OK;
+    }
+    // data every chunk reads, to the device once
+    int fixed(const void *src, size_t n, const char **dev)
+    {
+        int rc;
+        if ((rc = ensure(e, d_fixed, n))) return rc;
+        RTCHK(rt_h2d(d_fixed.p, src, n, e->stream));
+        *dev = (const char *)d_fixed.p;
+        return C2B_OK;
+    }
+    // d_out[0 .. n) to pinned host memory once the stream's work is done
+    int download(size_t n, const uint8_t **h)
+    {
+        if (!grow(h_out, h_out_cap, n)) return fail(e, C2B_E_CUDA, "packed rows: pinned allocation");
+        RTCHK(rt_d2h(h_out, d_out.p, n, e->stream));
+        RTCHK(rt_sync(e->stream));
+        *h = h_out;
+        return C2B_OK;
+    }
+};
+
+// the records of all chunks of a record pass, in row order
+struct RecordSink { std::vector<uint8_t> keys; std::vector<int64_t> rec_pos, rec_w; };
+
+// One chunk of m rows through a record pass (c2b_vcf.cuh, c2b_base_edit.cuh), P's inputs set: the size pass notes every row's
+// records, bytes and exception, a one-warp scan places them and finds the first exception, the write pass builds the records in
+// d_out and, after them, `extra` bytes of per-row output (*extra_out: their pinned host copy, at the P.* pointer that `write`
+// sets from its second argument).  -> C2B_OK; 1 with first[0..2] = chunk row, kind, value of the chunk's first exception; or an
+// error code.
+template <class PT, class Size, class Write>
+static int record_chunk(c2b_engine *e, ChunkPipe &cp, PT &P, int64_t m, size_t extra, Size size_pass, Write write_pass,
+                        RecordSink &S, int64_t *first, const uint8_t **extra_out)
+{
+    auto al = ChunkPipe::al;
+    // per row: nrec | nbytes | err (2) | rec_base (m + 1) | key_off (m + 1) | first (3)
+    const size_t l_nrec = 0, l_nbytes = al((size_t)m * 8), l_err = l_nbytes + al((size_t)m * 8), l_rb = l_err + al((size_t)m * 16),
+                 l_ko = l_rb + al((size_t)(m + 1) * 8), l_first = l_ko + al((size_t)(m + 1) * 8), l_end = l_first + 3 * 8;
+    int rc;
+    if ((rc = ensure(e, cp.d_len, l_end))) return rc;
+    char *dl = (char *)cp.d_len.p;
+    P.nrec = (int64_t *)(dl + l_nrec); P.nbytes = (int64_t *)(dl + l_nbytes); P.err = (int64_t *)(dl + l_err);
+    P.rec_base = (const int64_t *)(dl + l_rb); P.key_off = (const int64_t *)(dl + l_ko);
+    int64_t tot[2] = {0, 0};
+    first[0] = -1; first[1] = 0; first[2] = 0;
+    size_pass(P);
+#ifndef C2B_EMU
+    c2b_vcf_scan_kernel<<<1, 32, 0, e->stream>>>(P.nrec, (int64_t *)P.rec_base, P.nbytes, (int64_t *)P.key_off, P.err,
+                                                 (int64_t *)(dl + l_first), m);
+    RTCHK(cudaGetLastError());
+    RTCHK(rt_d2h(first, dl + l_first, 24, e->stream));
+    RTCHK(rt_d2h(&tot[0], P.rec_base + m, 8, e->stream));
+    RTCHK(rt_d2h(&tot[1], P.key_off + m, 8, e->stream));
+    RTCHK(rt_sync(e->stream));
+#else
+    emu::run_warp([&]() {
+        c2b::ann::scan_sizes(P.nrec, (int64_t *)P.rec_base, m);
+        c2b::ann::scan_sizes(P.nbytes, (int64_t *)P.key_off, m);
+        c2b::vcf::first_error(P.err, m, (int64_t *)(dl + l_first));
+    });
+    memcpy(first, dl + l_first, 24);
+    tot[0] = P.rec_base[m]; tot[1] = P.key_off[m];
+#endif
+    if (first[0] >= 0) return 1;
+    const size_t o_keys = 0, o_rpos = al((size_t)tot[1]), o_rw = o_rpos + al((size_t)tot[0] * 8), o_x = o_rw + al((size_t)tot[0] * 8),
+                 out_end = o_x + extra;
+    if ((rc = ensure(e, cp.d_out, out_end + 16))) return rc;
+    char *dout = (char *)cp.d_out.p;
+    P.keys = (uint8_t *)(dout + o_keys); P.rec_pos = (int64_t *)(dout + o_rpos); P.rec_w = (int64_t *)(dout + o_rw);
+    write_pass(P, dout + o_x);
+#ifndef C2B_EMU
+    RTCHK(cudaGetLastError());
+#endif
+    const uint8_t *h;
+    if ((rc = cp.download(out_end, &h))) return rc;
+    const int64_t kb = (int64_t)S.keys.size();
+    S.keys.insert(S.keys.end(), h + o_keys, h + o_keys + tot[1]);
+    const int64_t *hp = (const int64_t *)(h + o_rpos), *hw = (const int64_t *)(h + o_rw);
+    for (int64_t i = 0; i < tot[0]; i++) S.rec_pos.push_back(kb + hp[i]);
+    S.rec_w.insert(S.rec_w.end(), hw, hw + tot[0]);
+    if (extra_out) *extra_out = h + o_x;
+    return C2B_OK;
+}
+
+// every offset array starts at 0 and does not decrease
+static bool offsets_ok(const int64_t *const *offs, int n_offs, int64_t n_rows)
+{
+    for (int c = 0; c < n_offs; c++) {
+        if (offs[c][0] != 0) return false;
+        for (int64_t r = 0; r < n_rows; r++) if (offs[c][r + 1] < offs[c][r]) return false;
+    }
+    return true;
+}
+
+#ifndef C2B_EMU
+static int row_grid(int64_t m) { return (int)std::min<int64_t>((m + 7) / 8, 8192); }
+#endif
+
+extern "C" {
+
+// --vcf_output edit counts (c2b_vcf.cuh) for packed allele rows in chunks (ChunkPipe, record_chunk).  The records of all chunks
+// are then summed on the host (c2b_vcf_sum_records).
 int c2b_vcf_edit_counts(c2b_engine *e, int64_t n_rows, const int32_t *chrom, const int64_t *pos, const int64_t *reads,
                         const uint8_t *ref, const int64_t *ref_off, const uint8_t *aln, const int64_t *aln_off,
                         const int64_t *rp, const int64_t *rp_off, const int64_t *del, const int64_t *del_off,
@@ -1776,127 +1929,62 @@ int c2b_vcf_edit_counts(c2b_engine *e, int64_t n_rows, const int32_t *chrom, con
     *out = nullptr;
     err[0] = -1; err[1] = 0; err[2] = 0;
     const int64_t *offs[7] = {ref_off, aln_off, rp_off, del_off, ins_off, isz_off, sub_off};
-    for (const int64_t *o : offs) {
-        if (o[0] != 0) return fail(e, C2B_E_ARG, "c2b_vcf_edit_counts: offsets must start at 0");
-        for (int64_t r = 0; r < n_rows; r++) if (o[r + 1] < o[r]) return fail(e, C2B_E_ARG, "c2b_vcf_edit_counts: offsets must not decrease");
-    }
+    if (!offsets_ok(offs, 7, n_rows)) return fail(e, C2B_E_ARG, "c2b_vcf_edit_counts: offsets must start at 0 and not decrease");
     if (n_rows && (!chrom || !pos || !reads || (ref_off[n_rows] && !ref) || (aln_off[n_rows] && !aln) || (rp_off[n_rows] && !rp) ||
                    (del_off[n_rows] && !del) || (ins_off[n_rows] && !ins) || (isz_off[n_rows] && !isz) || (sub_off[n_rows] && !sub)))
         return fail(e, C2B_E_ARG, "c2b_vcf_edit_counts: row arrays missing");
     if (chunk <= 0) chunk = 1 << 14;
     const auto t0 = std::chrono::steady_clock::now();
-    auto al = [](size_t x) { return (x + 255) & ~(size_t)255; };
-    DevBuf d_in, d_len, d_out;
-    uint8_t *h_in = nullptr, *h_out = nullptr; size_t h_in_cap = 0, h_out_cap = 0;
-    auto cleanup = [&]() { rt_free(d_in.p); rt_free(d_len.p); rt_free(d_out.p); rt_host_free(h_in); rt_host_free(h_out); };
-    auto grow_host = [](uint8_t *&p, size_t &cap, size_t n) {
-        if (n <= cap) return true;
-        rt_host_free(p); cap = n + n / 4 + 4096; p = (uint8_t *)rt_host_alloc(cap);
-        return p != nullptr;
-    };
-    std::vector<uint8_t> keys;                                   // every record of every chunk, in row order
-    std::vector<int64_t> rec_pos, rec_w;
-    auto one_chunk = [&](int64_t r0) -> int {
-        const int64_t r1 = std::min(n_rows, r0 + chunk), m = r1 - r0;
-        // chunk input layout (device): chrom | pos | reads | then per column its values and its offsets rebased to the chunk
-        const void *col[7] = {ref, aln, rp, del, ins, isz, sub};
-        const size_t width[7] = {1, 1, 8, 16, 16, 8, 8};
-        size_t o_chrom = 0, o_pos = al((size_t)m * 4), o_reads = o_pos + al((size_t)m * 8), o = o_reads + al((size_t)m * 8);
-        size_t o_val[7], o_off[7];
-        for (int c = 0; c < 7; c++) {
-            o_val[c] = o; o += al((size_t)(offs[c][r1] - offs[c][r0]) * width[c]);
-            o_off[c] = o; o += al((size_t)(m + 1) * 8);
-        }
-        const size_t o_end = o;
-        if (!grow_host(h_in, h_in_cap, o_end)) return fail(e, C2B_E_CUDA, "c2b_vcf_edit_counts: pinned allocation");
-        memcpy(h_in + o_chrom, chrom + r0, (size_t)m * 4);
-        memcpy(h_in + o_pos, pos + r0, (size_t)m * 8);
-        memcpy(h_in + o_reads, reads + r0, (size_t)m * 8);
-        for (int c = 0; c < 7; c++) {
-            const int64_t b = offs[c][r0];
-            const size_t nb = (size_t)(offs[c][r1] - b) * width[c];
-            if (nb) memcpy(h_in + o_val[c], (const uint8_t *)col[c] + (size_t)b * width[c], nb);
-            int64_t *ho = (int64_t *)(h_in + o_off[c]);
-            for (int64_t r = 0; r <= m; r++) ho[r] = offs[c][r0 + r] - b;
-        }
-        // per row: nrec | nbytes | err (2) | rec_base (m + 1) | key_off (m + 1) | first (3)
-        const size_t l_nrec = 0, l_nbytes = al((size_t)m * 8), l_err = l_nbytes + al((size_t)m * 8), l_rb = l_err + al((size_t)m * 16),
-                     l_ko = l_rb + al((size_t)(m + 1) * 8), l_first = l_ko + al((size_t)(m + 1) * 8), l_end = l_first + 3 * 8;
-        int rc2;
-        if ((rc2 = ensure(e, d_in, o_end)) || (rc2 = ensure(e, d_len, l_end))) return rc2;
-        RTCHK(rt_h2d(d_in.p, h_in, o_end, e->stream));
-        char *di = (char *)d_in.p, *dl = (char *)d_len.p;
-        c2b::vcf::VParams P;
-        memset(&P, 0, sizeof P);
-        P.n = m;
-        P.chrom = (const int32_t *)(di + o_chrom); P.pos = (const int64_t *)(di + o_pos); P.reads = (const int64_t *)(di + o_reads);
-        P.ref = (const uint8_t *)(di + o_val[0]); P.ref_off = (const int64_t *)(di + o_off[0]);
-        P.aln = (const uint8_t *)(di + o_val[1]); P.aln_off = (const int64_t *)(di + o_off[1]);
-        P.rp = (const int64_t *)(di + o_val[2]); P.rp_off = (const int64_t *)(di + o_off[2]);
-        P.del = (const int64_t *)(di + o_val[3]); P.del_off = (const int64_t *)(di + o_off[3]);
-        P.ins = (const int64_t *)(di + o_val[4]); P.ins_off = (const int64_t *)(di + o_off[4]);
-        P.isz = (const int64_t *)(di + o_val[5]); P.isz_off = (const int64_t *)(di + o_off[5]);
-        P.sub = (const int64_t *)(di + o_val[6]); P.sub_off = (const int64_t *)(di + o_off[6]);
-        P.nrec = (int64_t *)(dl + l_nrec); P.nbytes = (int64_t *)(dl + l_nbytes); P.err = (int64_t *)(dl + l_err);
-        P.rec_base = (const int64_t *)(dl + l_rb); P.key_off = (const int64_t *)(dl + l_ko);
-        int64_t first[3] = {-1, 0, 0}, tot[2] = {0, 0};
-#ifndef C2B_EMU
-        const int grid = (int)std::min<int64_t>((m + 7) / 8, 8192);
-        c2b_vcf_size_kernel<<<grid, 256, 0, e->stream>>>(P);
-        c2b_vcf_scan_kernel<<<1, 32, 0, e->stream>>>(P.nrec, (int64_t *)P.rec_base, P.nbytes, (int64_t *)P.key_off, P.err,
-                                                     (int64_t *)(dl + l_first), m);
-        RTCHK(cudaGetLastError());
-        RTCHK(rt_d2h(first, dl + l_first, 24, e->stream));
-        RTCHK(rt_d2h(&tot[0], P.rec_base + m, 8, e->stream));
-        RTCHK(rt_d2h(&tot[1], P.key_off + m, 8, e->stream));
-        RTCHK(rt_sync(e->stream));
-#else
-        for (int64_t r = 0; r < m; r++) emu::run_warp([&]() { c2b::vcf::edits_one<false>(P, r); });
-        emu::run_warp([&]() {
-            c2b::ann::scan_sizes(P.nrec, (int64_t *)P.rec_base, m);
-            c2b::ann::scan_sizes(P.nbytes, (int64_t *)P.key_off, m);
-            c2b::vcf::first_error(P.err, m, (int64_t *)(dl + l_first));
-        });
-        memcpy(first, dl + l_first, 24);
-        tot[0] = P.rec_base[m]; tot[1] = P.key_off[m];
-#endif
-        if (first[0] >= 0) {
-            static const char *what[5] = {"", "KeyError", "ValueError: value is not in list", "IndexError: string index out of range",
-                                          "ValueError: max() iterable argument is empty"};
-            err[0] = r0 + first[0]; err[1] = first[1]; err[2] = first[2];
-            char msg[160];
-            snprintf(msg, sizeof msg, "c2b_vcf_edit_counts: row %lld raises %s (value %lld)", (long long)err[0],
-                     what[first[1] >= 1 && first[1] <= 4 ? first[1] : 0], (long long)err[2]);
-            return fail(e, C2B_E_ARG, msg);
-        }
-        const size_t o_keys = 0, o_rpos = al((size_t)tot[1]), o_rw = o_rpos + al((size_t)tot[0] * 8), out_end = o_rw + (size_t)tot[0] * 8;
-        if ((rc2 = ensure(e, d_out, out_end + 16))) return rc2;
-        char *dout = (char *)d_out.p;
-        P.keys = (uint8_t *)(dout + o_keys); P.rec_pos = (int64_t *)(dout + o_rpos); P.rec_w = (int64_t *)(dout + o_rw);
-#ifndef C2B_EMU
-        c2b_vcf_write_kernel<<<grid, 256, 0, e->stream>>>(P);
-        RTCHK(cudaGetLastError());
-#else
-        for (int64_t r = 0; r < m; r++) emu::run_warp([&]() { c2b::vcf::edits_one<true>(P, r); });
-#endif
-        if (!grow_host(h_out, h_out_cap, out_end)) return fail(e, C2B_E_CUDA, "c2b_vcf_edit_counts: pinned allocation");
-        RTCHK(rt_d2h(h_out, dout, out_end, e->stream));
-        RTCHK(rt_sync(e->stream));
-        const int64_t kb = (int64_t)keys.size();
-        keys.insert(keys.end(), h_out + o_keys, h_out + o_keys + tot[1]);
-        const int64_t *hp = (const int64_t *)(h_out + o_rpos), *hw = (const int64_t *)(h_out + o_rw);
-        for (int64_t i = 0; i < tot[0]; i++) rec_pos.push_back(kb + hp[i]);
-        rec_w.insert(rec_w.end(), hw, hw + tot[0]);
-        return C2B_OK;
-    };
+    const RowCol cols[10] = {{chrom, nullptr, 4}, {pos, nullptr, 8}, {reads, nullptr, 8}, {ref, ref_off, 1}, {aln, aln_off, 1},
+                             {rp, rp_off, 8}, {del, del_off, 16}, {ins, ins_off, 16}, {isz, isz_off, 8}, {sub, sub_off, 8}};
+    RecordSink S;
     int rc = C2B_OK;
-    for (int64_t r0 = 0; !rc && r0 < n_rows; r0 += chunk) rc = one_chunk(r0);
-    cleanup();
+    {
+        ChunkPipe cp(e);
+        for (int64_t r0 = 0; !rc && r0 < n_rows; r0 += chunk) {
+            const int64_t r1 = std::min(n_rows, r0 + chunk), m = r1 - r0;
+            const char *d[10]; const int64_t *o[10];
+            if ((rc = cp.upload(cols, 10, r0, r1, d, o))) break;
+            c2b::vcf::VParams P;
+            memset(&P, 0, sizeof P);
+            P.n = m;
+            P.chrom = (const int32_t *)d[0]; P.pos = (const int64_t *)d[1]; P.reads = (const int64_t *)d[2];
+            P.ref = (const uint8_t *)d[3]; P.ref_off = o[3]; P.aln = (const uint8_t *)d[4]; P.aln_off = o[4];
+            P.rp = (const int64_t *)d[5]; P.rp_off = o[5]; P.del = (const int64_t *)d[6]; P.del_off = o[6];
+            P.ins = (const int64_t *)d[7]; P.ins_off = o[7]; P.isz = (const int64_t *)d[8]; P.isz_off = o[8];
+            P.sub = (const int64_t *)d[9]; P.sub_off = o[9];
+            auto size_pass = [&](const c2b::vcf::VParams &Q) {
+#ifndef C2B_EMU
+                c2b_vcf_size_kernel<<<row_grid(m), 256, 0, e->stream>>>(Q);
+#else
+                for (int64_t r = 0; r < m; r++) emu::run_warp([&]() { c2b::vcf::edits_one<false>(Q, r); });
+#endif
+            };
+            auto write_pass = [&](const c2b::vcf::VParams &Q, char *) {
+#ifndef C2B_EMU
+                c2b_vcf_write_kernel<<<row_grid(m), 256, 0, e->stream>>>(Q);
+#else
+                for (int64_t r = 0; r < m; r++) emu::run_warp([&]() { c2b::vcf::edits_one<true>(Q, r); });
+#endif
+            };
+            int64_t first[3];
+            rc = record_chunk(e, cp, P, m, 0, size_pass, write_pass, S, first, nullptr);
+            if (rc == 1) {
+                static const char *what[5] = {"", "KeyError", "ValueError: value is not in list", "IndexError: string index out of range",
+                                              "ValueError: max() iterable argument is empty"};
+                err[0] = r0 + first[0]; err[1] = first[1]; err[2] = first[2];
+                char msg[160];
+                snprintf(msg, sizeof msg, "c2b_vcf_edit_counts: row %lld raises %s (value %lld)", (long long)err[0],
+                         what[first[1] >= 1 && first[1] <= 4 ? first[1] : 0], (long long)err[2]);
+                rc = fail(e, C2B_E_ARG, msg);
+            }
+        }
+    }
     if (rc) return rc;
     const auto t1 = std::chrono::steady_clock::now();
-    rec_pos.push_back((int64_t)keys.size());
+    S.rec_pos.push_back((int64_t)S.keys.size());
     std::unique_ptr<c2b_vcf_counts> V(new c2b_vcf_counts());
-    if (!c2b_vcf_sum_records(keys.data(), rec_pos.data(), rec_w.data(), (int64_t)rec_w.size(), V.get()))
+    if (!c2b_vcf_sum_records(S.keys.data(), S.rec_pos.data(), S.rec_w.data(), (int64_t)S.rec_w.size(), V.get()))
         return fail(e, C2B_E_LIMIT, "c2b_vcf_edit_counts: a summed #Reads leaves int64");
     const auto t2 = std::chrono::steady_clock::now();
     V->device_ms = std::chrono::duration<double, std::milli>(t1 - t0).count();
@@ -1915,6 +2003,256 @@ int c2b_vcf_timings(const c2b_vcf_counts *v, double *device_ms, double *sum_ms)
 {
     if (!v || !device_ms || !sum_ms) return C2B_E_ARG;
     *device_ms = v->device_ms; *sum_ms = v->sum_ms;
+    return C2B_OK;
+}
+
+}  // extern "C"
+
+// --base_editor_output upset counts: the summed keys (tag byte | key text, c2b_base_edit.cuh) and the totals of
+// c2b_be_upset_totals
+struct c2b_be_upset {
+    c2b_vcf_counts keys;
+    std::vector<int64_t> totals;
+};
+
+// --base_editor_output quilt table: the projections of all rows (arena), Reference_Sequence projections (nuc repeated) and the
+// sorted groups, whose strings point into them
+struct c2b_be_quilt {
+    std::vector<uint8_t> arena, nucs;
+    std::vector<c2b_cut_group> groups;
+    double device_ms = 0, group_ms = 0;
+};
+
+extern "C" {
+
+// get_upset_plot_counts (c2b_base_edit.cuh) for packed allele rows in chunks (ChunkPipe, record_chunk); the records are summed on
+// the host (c2b_vcf_sum_records), the category codes give the per-position counts and the totals.
+int c2b_be_upset_counts(c2b_engine *e, int64_t n_rows, const uint8_t *flags, const int64_t *reads, const uint8_t *ref,
+                        const int64_t *ref_off, const uint8_t *aln, const int64_t *aln_off, int32_t n_targets, const int64_t *tpos,
+                        const uint8_t *tstr, const int64_t *toff, int64_t chunk, int64_t *err, c2b_be_upset **out)
+{
+    if (!e || !out || !err || n_rows < 0 || !ref_off || !aln_off || n_targets < 0 || (n_targets && (!tpos || !toff)))
+        return fail(e, C2B_E_ARG, "c2b_be_upset_counts: bad argument");
+    *out = nullptr;
+    err[0] = -1; err[1] = 0;
+    const int64_t *offs[2] = {ref_off, aln_off};
+    if (!offsets_ok(offs, 2, n_rows)) return fail(e, C2B_E_ARG, "c2b_be_upset_counts: offsets must start at 0 and not decrease");
+    if (n_rows && (!flags || !reads || (ref_off[n_rows] && !ref) || (aln_off[n_rows] && !aln)))
+        return fail(e, C2B_E_ARG, "c2b_be_upset_counts: row arrays missing");
+    const int nt = n_targets;
+    const int64_t ts = nt ? toff[2 * nt] : 0;
+    if (nt && (toff[0] != 0 || (ts && !tstr))) return fail(e, C2B_E_ARG, "c2b_be_upset_counts: target strings missing");
+    for (int k = 0; k < 2 * nt; k++) if (toff[k + 1] < toff[k]) return fail(e, C2B_E_ARG, "c2b_be_upset_counts: target offsets decrease");
+    if (chunk <= 0) chunk = 1 << 14;
+    const auto t0 = std::chrono::steady_clock::now();
+    const RowCol cols[4] = {{flags, nullptr, 1}, {reads, nullptr, 8}, {ref, ref_off, 1}, {aln, aln_off, 1}};
+    // targets: positions (nt) | offsets (2 nt + 1) | strings
+    std::vector<uint8_t> fixed((size_t)(8 * nt + 8 * (2 * nt + 1) + ts));
+    if (nt) {
+        memcpy(fixed.data(), tpos, (size_t)nt * 8);
+        memcpy(fixed.data() + 8 * nt, toff, (size_t)(2 * nt + 1) * 8);
+        if (ts) memcpy(fixed.data() + 8 * nt + 8 * (2 * nt + 1), tstr, (size_t)ts);
+    }
+    RecordSink S;
+    std::vector<uint8_t> codes((size_t)n_rows * nt);
+    int rc = C2B_OK;
+    {
+        ChunkPipe cp(e);
+        const char *df = nullptr;
+        rc = cp.fixed(fixed.data(), fixed.size(), &df);
+        for (int64_t r0 = 0; !rc && r0 < n_rows; r0 += chunk) {
+            const int64_t r1 = std::min(n_rows, r0 + chunk), m = r1 - r0;
+            const char *d[4]; const int64_t *o[4];
+            if ((rc = cp.upload(cols, 4, r0, r1, d, o))) break;
+            c2b::be::UParams P;
+            memset(&P, 0, sizeof P);
+            P.n = m; P.flags = (const uint8_t *)d[0]; P.reads = (const int64_t *)d[1];
+            P.ref = (const uint8_t *)d[2]; P.ref_off = o[2]; P.aln = (const uint8_t *)d[3]; P.aln_off = o[3];
+            P.nt = nt; P.tpos = (const int64_t *)df; P.toff = (const int64_t *)(df + 8 * nt);
+            P.tstr = (const uint8_t *)(df + 8 * nt + 8 * (2 * nt + 1));
+            auto size_pass = [&](const c2b::be::UParams &Q) {
+#ifndef C2B_EMU
+                c2b_be_upset_size_kernel<<<row_grid(m), 256, 0, e->stream>>>(Q);
+#else
+                for (int64_t r = 0; r < m; r++) emu::run_warp([&]() { c2b::be::upset_one<false>(Q, r); });
+#endif
+            };
+            auto write_pass = [&](c2b::be::UParams &Q, char *x) {
+                Q.codes = (uint8_t *)x;
+#ifndef C2B_EMU
+                c2b_be_upset_write_kernel<<<row_grid(m), 256, 0, e->stream>>>(Q);
+#else
+                for (int64_t r = 0; r < m; r++) emu::run_warp([&]() { c2b::be::upset_one<true>(Q, r); });
+#endif
+            };
+            int64_t first[3];
+            const uint8_t *hc = nullptr;
+            rc = record_chunk(e, cp, P, m, (size_t)m * nt, size_pass, write_pass, S, first, &hc);
+            if (rc == 1) {
+                err[0] = r0 + first[0]; err[1] = first[1];
+                char msg[160];
+                snprintf(msg, sizeof msg, "c2b_be_upset_counts: row %lld raises IndexError: string index out of range", (long long)err[0]);
+                rc = fail(e, C2B_E_ARG, msg);
+            } else if (!rc && m * nt) {
+                memcpy(codes.data() + (size_t)r0 * nt, hc, (size_t)(m * nt));
+            }
+        }
+    }
+    if (rc) return rc;
+    const auto t1 = std::chrono::steady_clock::now();
+    std::unique_ptr<c2b_be_upset> U(new c2b_be_upset());
+    S.rec_pos.push_back((int64_t)S.keys.size());
+    bool ok = c2b_vcf_sum_records(S.keys.data(), S.rec_pos.data(), S.rec_w.data(), (int64_t)S.rec_w.size(), &U->keys);
+    // totals (C2B_BE_T_*), then per category (C2B_BE_CAT_*) the #Reads of every target position
+    std::vector<int64_t> &T = U->totals;
+    T.assign((size_t)(10 + 5 * nt), 0);
+    int64_t *pc = T.data() + 10;
+    auto add = [&](int64_t &a, int64_t b) { if (__builtin_add_overflow(a, b, &a)) ok = false; };
+    T[0] = n_rows;
+    for (int64_t r = 0; r < n_rows; r++) {
+        const int64_t w = reads[r];
+        add(T[1], w);
+        if (!(flags[r] & 1)) continue;
+        T[2]++;
+        add(T[3], w);
+        const uint8_t *c = codes.data() + (size_t)r * nt;
+        bool all_r = true, all_t = true;
+        for (int t = 0; t < nt; t++) {
+            add(pc[(size_t)c[t] * nt + t], w);
+            all_r = all_r && c[t] == c2b::be::CAT_R;
+            all_t = all_t && c[t] == c2b::be::CAT_T;
+        }
+        add(T[4 + 2 * (all_r ? 0 : all_t ? 1 : 2) + ((flags[r] & 2) ? 1 : 0)], w);
+    }
+    if (!ok) return fail(e, C2B_E_LIMIT, "c2b_be_upset_counts: a summed #Reads leaves int64");
+    const auto t2 = std::chrono::steady_clock::now();
+    U->keys.device_ms = std::chrono::duration<double, std::milli>(t1 - t0).count();
+    U->keys.sum_ms = std::chrono::duration<double, std::milli>(t2 - t1).count();
+    *out = U.release();
+    return C2B_OK;
+}
+
+void c2b_be_upset_free(c2b_be_upset *u) { delete u; }
+int64_t c2b_be_upset_n(const c2b_be_upset *u) { return u ? (int64_t)u->keys.reads.size() : 0; }
+const uint8_t *c2b_be_upset_keys(const c2b_be_upset *u) { return u ? u->keys.keys.get() : nullptr; }
+const int64_t *c2b_be_upset_key_offsets(const c2b_be_upset *u) { return u ? u->keys.key_off.data() : nullptr; }
+const int64_t *c2b_be_upset_reads(const c2b_be_upset *u) { return u ? u->keys.reads.data() : nullptr; }
+const int64_t *c2b_be_upset_totals(const c2b_be_upset *u) { return u ? u->totals.data() : nullptr; }
+int c2b_be_upset_timings(const c2b_be_upset *u, double *device_ms, double *sum_ms)
+{
+    if (!u || !device_ms || !sum_ms) return C2B_E_ARG;
+    *device_ms = u->keys.device_ms; *sum_ms = u->keys.sum_ms;
+    return C2B_OK;
+}
+
+// get_base_edit_dataframe_around_cut (c2b_base_edit.cuh) for packed allele rows in chunks (ChunkPipe): one pass writes each
+// row's projection at its Reference_Sequence offset, its length and its error; the projections are then grouped and sorted on
+// the host (c2b_group_around_cut).
+int c2b_be_quilt_table(c2b_engine *e, int64_t n_rows, int32_t nuc, const uint8_t *ref, const int64_t *ref_off, const uint8_t *aln,
+                 const int64_t *aln_off, const uint8_t *unedited, const int64_t *n_deleted, const int64_t *n_inserted,
+                 const int64_t *n_mutated, const int64_t *reads, const double *pct, int64_t chunk, int64_t *err, c2b_be_quilt **out)
+{
+    if (!e || !out || !err || n_rows < 0 || !ref_off || !aln_off || nuc > 255) return fail(e, C2B_E_ARG, "c2b_be_quilt_table: bad argument");
+    *out = nullptr;
+    err[0] = -1;
+    const int64_t *offs[2] = {ref_off, aln_off};
+    if (!offsets_ok(offs, 2, n_rows)) return fail(e, C2B_E_ARG, "c2b_be_quilt_table: offsets must start at 0 and not decrease");
+    if (n_rows && (!unedited || !n_deleted || !n_inserted || !n_mutated || !reads || !pct || (ref_off[n_rows] && !ref) ||
+                   (aln_off[n_rows] && !aln)))
+        return fail(e, C2B_E_ARG, "c2b_be_quilt_table: row arrays missing");
+    if (chunk <= 0) chunk = 1 << 14;
+    const auto t0 = std::chrono::steady_clock::now();
+    const RowCol cols[2] = {{ref, ref_off, 1}, {aln, aln_off, 1}};
+    std::unique_ptr<c2b_be_quilt> Q(new c2b_be_quilt());
+    std::vector<int64_t> plen((size_t)n_rows), pstart((size_t)n_rows);
+    int rc = C2B_OK;
+    {
+        ChunkPipe cp(e);
+        auto al = ChunkPipe::al;
+        for (int64_t r0 = 0; !rc && r0 < n_rows; r0 += chunk) {
+            const int64_t r1 = std::min(n_rows, r0 + chunk), m = r1 - r0, rb = ref_off[r1] - ref_off[r0];
+            const char *d[2]; const int64_t *o[2];
+            if ((rc = cp.upload(cols, 2, r0, r1, d, o))) break;
+            // out: projections (at the chunk's Reference_Sequence offsets) | len (m) | err (m)
+            const size_t o_len = al((size_t)rb), o_err = o_len + al((size_t)m * 8), o_end = o_err + (size_t)m * 8;
+            if ((rc = ensure(e, cp.d_out, o_end + 16))) break;
+            char *dout = (char *)cp.d_out.p;
+            c2b::be::QParams P;
+            memset(&P, 0, sizeof P);
+            P.n = m; P.nuc = nuc; P.ref = (const uint8_t *)d[0]; P.ref_off = o[0]; P.aln = (const uint8_t *)d[1]; P.aln_off = o[1];
+            P.out = (uint8_t *)dout; P.len = (int64_t *)(dout + o_len); P.err = (int64_t *)(dout + o_err);
+#ifndef C2B_EMU
+            c2b_be_quilt_kernel<<<row_grid(m), 256, 0, e->stream>>>(P);
+            if (cudaGetLastError() != cudaSuccess) { rc = fail(e, C2B_E_CUDA, "c2b_be_quilt_table: launch failed"); break; }
+#else
+            for (int64_t r = 0; r < m; r++) emu::run_warp([&]() { c2b::be::quilt_one(P, r); });
+#endif
+            const uint8_t *h;
+            if ((rc = cp.download(o_end, &h))) break;
+            const int64_t *hl = (const int64_t *)(h + o_len), *he = (const int64_t *)(h + o_err);
+            for (int64_t r = 0; r < m; r++)
+                if (he[r]) {
+                    err[0] = r0 + r;
+                    char msg[160];
+                    snprintf(msg, sizeof msg, "c2b_be_quilt_table: row %lld raises IndexError: string index out of range", (long long)err[0]);
+                    rc = fail(e, C2B_E_ARG, msg);
+                    break;
+                }
+            if (rc) break;
+            for (int64_t r = 0; r < m; r++) {
+                const int64_t s = ref_off[r0 + r] - ref_off[r0];
+                pstart[(size_t)(r0 + r)] = (int64_t)Q->arena.size();
+                plen[(size_t)(r0 + r)] = hl[r];
+                Q->arena.insert(Q->arena.end(), h + s, h + s + hl[r]);
+            }
+        }
+    }
+    if (rc) return rc;
+    const auto t1 = std::chrono::steady_clock::now();
+    int64_t longest = 0;
+    for (int64_t r = 0; r < n_rows; r++) longest = std::max(longest, plen[(size_t)r]);
+    Q->nucs.assign((size_t)longest + 1, (uint8_t)(nuc < 0 ? 0 : nuc));
+    std::vector<c2b_cut_group> rows((size_t)n_rows);
+    for (int64_t r = 0; r < n_rows; r++) {
+        c2b_cut_group &G = rows[(size_t)r];
+        G.seq = Q->arena.data() + pstart[(size_t)r]; G.ref = Q->nucs.data(); G.len = plen[(size_t)r];
+        G.unedited = unedited[r] ? 1 : 0; G.ndel = n_deleted[r]; G.nins = n_inserted[r]; G.nmut = n_mutated[r];
+        G.reads = reads[r]; G.pct = pct[r];
+    }
+    Q->groups = c2b_group_around_cut(rows);
+    const auto t2 = std::chrono::steady_clock::now();
+    Q->device_ms = std::chrono::duration<double, std::milli>(t1 - t0).count();
+    Q->group_ms = std::chrono::duration<double, std::milli>(t2 - t1).count();
+    *out = Q.release();
+    return C2B_OK;
+}
+
+void c2b_be_quilt_free(c2b_be_quilt *q) { delete q; }
+int64_t c2b_be_quilt_n(const c2b_be_quilt *q) { return q ? (int64_t)q->groups.size() : 0; }
+int64_t c2b_be_quilt_bytes(const c2b_be_quilt *q)
+{
+    int64_t n = 0;
+    if (q) for (const c2b_cut_group &G : q->groups) n += G.len;
+    return n;
+}
+int c2b_be_quilt_fetch(const c2b_be_quilt *q, uint8_t *seq, int64_t *seq_off, uint8_t *unedited, int64_t *n_deleted, int64_t *n_inserted,
+                       int64_t *n_mutated, int64_t *reads, double *pct)
+{
+    if (!q || !seq_off || !unedited || !n_deleted || !n_inserted || !n_mutated || !reads || !pct) return C2B_E_ARG;
+    int64_t o = 0;
+    seq_off[0] = 0;
+    for (size_t g = 0; g < q->groups.size(); g++) {
+        const c2b_cut_group &G = q->groups[g];
+        if (G.len) { if (!seq) return C2B_E_ARG; memcpy(seq + o, G.seq, (size_t)G.len); }
+        o += G.len; seq_off[g + 1] = o;
+        unedited[g] = G.unedited; n_deleted[g] = G.ndel; n_inserted[g] = G.nins; n_mutated[g] = G.nmut; reads[g] = G.reads; pct[g] = G.pct;
+    }
+    return C2B_OK;
+}
+int c2b_be_quilt_timings(const c2b_be_quilt *q, double *device_ms, double *group_ms)
+{
+    if (!q || !device_ms || !group_ms) return C2B_E_ARG;
+    *device_ms = q->device_ms; *group_ms = q->group_ms;
     return C2B_OK;
 }
 

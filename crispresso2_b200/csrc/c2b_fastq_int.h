@@ -52,6 +52,17 @@ struct c2b_vcf_counts {
 // false when a sum leaves int64
 bool c2b_vcf_sum_records(const uint8_t *arena, const int64_t *off, const int64_t *w, int64_t n, c2b_vcf_counts *out);
 
+// One row, or one group, of the tables around the cut before pandas' groupby (get_dataframe_around_cut_asymmetrical,
+// get_base_edit_dataframe_around_cut): Aligned_Sequence seq[0 .. len) and Reference_Sequence ref[0 .. len), the other key columns,
+// #Reads and %Reads (comp: the Kahan compensation of a group's sum)
+struct c2b_cut_group {
+    const uint8_t *seq, *ref; int64_t len;
+    uint8_t unedited; int64_t ndel, nins, nmut;
+    int64_t reads; double pct, comp;
+};
+// groupby over the six key columns with .sum() in row order, sorted as the reference sorts the result (c2b_alleles.cpp)
+std::vector<c2b_cut_group> c2b_group_around_cut(const std::vector<c2b_cut_group> &rows);
+
 // whole file into memory (c2b_fastq.cpp): plain read / gzip inflate (blocked gzip: all host threads)
 bool c2b_fastq_read_gz(const char *path, c2b_bytes &buf, std::string &err);
 void c2b_fastq_set_error(const std::string &m);

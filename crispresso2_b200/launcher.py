@@ -19,6 +19,11 @@ What is re-bound (INTEGRATION.md section 2), nothing else of the reference chang
   * writers.vcf.build_edit_counts (module global, called by vcf.write_vcf_file, writers/vcf.py:317; --vcf_output,
     CRISPRessoCORE.py:4487-4496)   -> crispresso2_b200.vcf.build_edit_counts on the launcher's engine, in single-process runs
     and under torchrun alike (every rank runs main() over the same cache)
+  * plots.data_prep.get_upset_plot_counts (module global, called by prep_base_edit_upset, data_prep.py:2141) and its copy
+    CRISPRessoCORE.get_upset_plot_counts (:209-327)   -> crispresso2_b200.base_edit.get_upset_plot_counts on the launcher's engine
+  * CRISPRessoShared.get_base_edit_dataframe_around_cut (called by data_prep.prep_base_edit_quilt, :1675)
+    -> crispresso2_b200.base_edit.get_base_edit_dataframe_around_cut on the launcher's engine
+    (--base_editor_output, figures 10i and 10h; both in single-process runs and under torchrun alike)
 Under torchrun (WORLD_SIZE > 1) every rank runs the same command; process_fastq shards the unique reads over the ranks' GPUs
 and merges the count block with one all-reduce (core.process_fastq_sharded); rank 0's output directory is the result.
 
@@ -135,6 +140,18 @@ def bind(CORE=None, engine=None, lib_path=None):
         return vcf.build_edit_counts(df_alleles, amplicon_positions, engine=get_engine())
 
     CORE.vcf.build_edit_counts = build_edit_counts
+    # --base_editor_output: the upset keys and the quilt projections built on the GPU, summed / grouped natively (base_edit.py)
+    from . import base_edit
+
+    def get_upset_plot_counts(df_alleles, bp_substitutions_arr, wt_ref_name):
+        return base_edit.get_upset_plot_counts(df_alleles, bp_substitutions_arr, wt_ref_name, engine=get_engine())
+
+    def get_base_edit_dataframe_around_cut(df_alleles, conversion_nuc_inds):
+        return base_edit.get_base_edit_dataframe_around_cut(df_alleles, conversion_nuc_inds, engine=get_engine())
+
+    CORE.CRISPRessoPlotData.get_upset_plot_counts = get_upset_plot_counts
+    CORE.get_upset_plot_counts = get_upset_plot_counts
+    SH.get_base_edit_dataframe_around_cut = get_base_edit_dataframe_around_cut
     return CORE
 
 

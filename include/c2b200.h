@@ -493,6 +493,63 @@ int64_t        c2b_vcf_n_records(const c2b_vcf_counts *v);     /* records before
 /* wall time of the call's device pass with its copies, and of the host sum, in ms */
 int  c2b_vcf_timings(const c2b_vcf_counts *v, double *device_ms, double *sum_ms);
 
+/* ---- --base_editor_output allele tables (csrc/c2b_base_edit.cuh on the device; keys summed in csrc/c2b_fastq.cpp, groups in
+ * csrc/c2b_alleles.cpp) ----
+ * Rows come packed: Reference_Sequence / Aligned_Sequence bytes at ref_off / aln_off (n_rows + 1 offsets starting at 0), in chunks
+ * of `chunk` rows (<= 0: 16384) through pinned buffers on the engine's stream.
+ *
+ * c2b_be_upset_counts replaces: get_upset_plot_counts (CRISPResso2/plots/data_prep.py:1869-1988, identical copy
+ * CRISPRessoCORE.py:209-327) with get_refpos_values (data_prep.py:1816-1856).  Per row flags (bit 0: Reference_Name ==
+ * wt_ref_name, bit 1: n_deleted > 0 or n_inserted > 0) and #Reads; target t of bp_substitutions_arr at reference position
+ * tpos[t], its ref_base at tstr[toff[2t] .. toff[2t+1]) and mod_base at tstr[toff[2t+1] .. toff[2t+2]).
+ * Result: the distinct keys in first-seen order, key i at keys[key_off[i] .. key_off[i+1]) as a tag byte (0 binary, 1 category,
+ * 2 precise) followed by the reference's key text, with its summed #Reads; and the totals (C2B_BE_T_*, then for each category
+ * C2B_BE_CAT_* the n_targets per-position counts).  When a row on wt_ref_name has an empty Reference_Sequence or an
+ * Aligned_Sequence shorter than it (the reference raises IndexError: string index out of range), returns C2B_E_ARG with
+ * err[0..1] = the first such row, C2B_BE_E_STRING_INDEX; err[0] = -1 otherwise.  C2B_E_LIMIT: a sum leaves int64.         */
+#define C2B_BE_E_STRING_INDEX  1
+#define C2B_BE_CAT_R 0              /* reference_base_counts */
+#define C2B_BE_CAT_T 1              /* target_base_counts */
+#define C2B_BE_CAT_D 2              /* deletion_base_counts */
+#define C2B_BE_CAT_I 3              /* insertion_base_counts */
+#define C2B_BE_CAT_N 4              /* other_base_counts */
+/* totals: total_alleles, total_alleles_reads, total_alleles_on_ref, total_alleles_reads_on_ref, total_reference_noindel_reads,
+ * total_reference_indel_reads, total_target_noindel_reads, total_target_indel_reads, total_other_noindel_reads,
+ * total_other_indel_reads */
+#define C2B_BE_N_TOTALS 10
+typedef struct c2b_be_upset c2b_be_upset;
+int  c2b_be_upset_counts(c2b_engine *e, int64_t n_rows, const uint8_t *flags, const int64_t *reads, const uint8_t *ref,
+                         const int64_t *ref_off, const uint8_t *aln, const int64_t *aln_off, int32_t n_targets, const int64_t *tpos,
+                         const uint8_t *tstr, const int64_t *toff, int64_t chunk, int64_t *err, c2b_be_upset **out);
+void c2b_be_upset_free(c2b_be_upset *u);
+int64_t        c2b_be_upset_n(const c2b_be_upset *u);              /* distinct keys of the three kinds */
+const uint8_t *c2b_be_upset_keys(const c2b_be_upset *u);
+const int64_t *c2b_be_upset_key_offsets(const c2b_be_upset *u);    /* n + 1 */
+const int64_t *c2b_be_upset_reads(const c2b_be_upset *u);          /* summed #Reads per key */
+const int64_t *c2b_be_upset_totals(const c2b_be_upset *u);         /* C2B_BE_N_TOTALS + 5 * n_targets */
+/* wall time of the call's device pass with its copies, and of the host sums, in ms */
+int  c2b_be_upset_timings(const c2b_be_upset *u, double *device_ms, double *sum_ms);
+
+/* c2b_be_quilt replaces: get_base_edit_dataframe_around_cut with get_base_edit_row_around_cut (CRISPRessoShared.py:1472-1506):
+ * per row the Aligned_Sequence characters at the columns where Reference_Sequence holds `nuc` (-1: conversion_nuc_from is not one
+ * character, every projection is empty), then pandas' groupby over (projection, nuc * its length, unedited, n_deleted,
+ * n_inserted, n_mutated) with #Reads summed in int64 and %Reads with pandas' Kahan group_sum in row order, sorted by #Reads
+ * descending, then both strings ascending, in groupby's key order (the grouping of c2b_alleles_around_cut).  When a needed
+ * column lies past the end of Aligned_Sequence (IndexError: string index out of range), returns C2B_E_ARG with err[0] = the
+ * first such row; err[0] = -1 otherwise.                                                                                     */
+typedef struct c2b_be_quilt c2b_be_quilt;
+int  c2b_be_quilt_table(c2b_engine *e, int64_t n_rows, int32_t nuc, const uint8_t *ref, const int64_t *ref_off, const uint8_t *aln,
+                  const int64_t *aln_off, const uint8_t *unedited, const int64_t *n_deleted, const int64_t *n_inserted,
+                  const int64_t *n_mutated, const int64_t *reads, const double *pct, int64_t chunk, int64_t *err, c2b_be_quilt **out);
+void c2b_be_quilt_free(c2b_be_quilt *q);
+int64_t c2b_be_quilt_n(const c2b_be_quilt *q);                     /* groups */
+int64_t c2b_be_quilt_bytes(const c2b_be_quilt *q);                 /* summed length of the groups' projections */
+/* the groups in order: projection g at seq[seq_off[g] .. seq_off[g+1]) (seq_off: n + 1), the other key columns and the sums */
+int  c2b_be_quilt_fetch(const c2b_be_quilt *q, uint8_t *seq, int64_t *seq_off, uint8_t *unedited, int64_t *n_deleted,
+                        int64_t *n_inserted, int64_t *n_mutated, int64_t *reads, double *pct);
+/* wall time of the call's device pass with its copies, and of the host grouping, in ms */
+int  c2b_be_quilt_timings(const c2b_be_quilt *q, double *device_ms, double *group_ms);
+
 /* ---- paired-end merge mode (csrc/c2b_paired.cpp) ----
  * get_consensus_alignment_from_pairs (CRISPRessoCORE.py:829-985, get_greater_qual_nuc :801-826): the two mates' alignments to one
  * amplicon (aligned read, aligned amplicon, score, quality string of the read's bases) merged column by column into one aligned
