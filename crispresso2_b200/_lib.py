@@ -38,6 +38,8 @@ ST_TOO_LONG = 8
 VCF_E_KEY, VCF_E_NOT_IN_LIST, VCF_E_STRING_INDEX, VCF_E_EMPTY_MAX = 1, 2, 3, 4     # C2B_VCF_E_*: c2b_vcf_edit_counts' err[1]
 BE_E_STRING_INDEX = 1                                   # C2B_BE_E_*: c2b_be_upset_counts' err[1]
 BE_N_TOTALS = 10                                        # C2B_BE_N_TOTALS
+AA_MAX_Q = 32                                           # C2B_AA_MAX_Q: read alphabet of c2b_protein_align
+AA_E_NOT_IN_LIST, AA_E_CODON, AA_E_EMPTY, AA_E_UNDEFINED = 1, 2, 3, 4     # C2B_AA_E_*: c2b_amino_table's err[1]
 
 # count-block layout (enum order of c2b200.h)
 V_ALL_INS, V_ALL_INS_LEFT, V_ALL_DEL, V_ALL_SUB, V_INS, V_DEL, V_SUB, V_SUBBASE0 = range(8)
@@ -100,7 +102,9 @@ EXPORTS = ["c2b_create", "c2b_destroy", "c2b_last_error", "c2b_configure", "c2b_
            "c2b_vcf_keys", "c2b_vcf_key_offsets", "c2b_vcf_reads", "c2b_vcf_n_records", "c2b_vcf_timings",
            "c2b_be_upset_counts", "c2b_be_upset_free", "c2b_be_upset_n", "c2b_be_upset_keys", "c2b_be_upset_key_offsets",
            "c2b_be_upset_reads", "c2b_be_upset_totals", "c2b_be_upset_timings", "c2b_be_quilt_table", "c2b_be_quilt_free",
-           "c2b_be_quilt_n", "c2b_be_quilt_bytes", "c2b_be_quilt_fetch", "c2b_be_quilt_timings"]
+           "c2b_be_quilt_n", "c2b_be_quilt_bytes", "c2b_be_quilt_fetch", "c2b_be_quilt_timings", "c2b_protein_align",
+           "c2b_amino_table", "c2b_amino_free", "c2b_amino_n", "c2b_amino_bytes", "c2b_amino_ref_lens", "c2b_amino_fetch",
+           "c2b_amino_timings"]
 
 _cache = {}
 
@@ -290,5 +294,16 @@ def load(path=None):
     for name in ("c2b_be_upset_timings", "c2b_be_quilt_timings"):
         getattr(L, name).restype = C.c_int
         getattr(L, name).argtypes = [vp, C.POINTER(C.c_double), C.POINTER(C.c_double)]
+    L.c2b_protein_align.restype = C.c_int
+    L.c2b_protein_align.argtypes = [vp, C.c_char_p, i32, C.c_char_p, vp, i64, C.c_char_p, i32, vp, vp, i32, i32, vp, vp, vp]
+    L.c2b_amino_table.restype = C.c_int
+    L.c2b_amino_table.argtypes = [vp, i64, i64] + [vp] * 7 + [i32, i64, i64] + [vp] * 6 + [i64, vp, C.POINTER(vp)]
+    for name, rt in (("c2b_amino_free", None), ("c2b_amino_n", i64), ("c2b_amino_bytes", i64), ("c2b_amino_ref_lens", vp)):
+        getattr(L, name).restype = rt
+        getattr(L, name).argtypes = [vp]
+    L.c2b_amino_fetch.restype = C.c_int
+    L.c2b_amino_fetch.argtypes = [vp] * 10
+    L.c2b_amino_timings.restype = C.c_int
+    L.c2b_amino_timings.argtypes = [vp] + [C.POINTER(C.c_double)] * 3 + [C.POINTER(C.c_int64)]
     _cache[path] = L
     return L

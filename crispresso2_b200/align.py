@@ -3,7 +3,8 @@
   read_matrix(path)            Align.pyx:33-61
   make_matrix(...)             Align.pyx:63-99
   global_align(seqj, seqi, matrix, gap_incentive, gap_open=-1, gap_extend=-1) -> (str, str, float)
-                               Align.pyx:101-434 -- runs on the GPU through c2b_global_align.
+                               Align.pyx:101-434 -- runs on the GPU through c2b_global_align, or through c2b_protein_align
+                               when the read has 9 to 32 distinct symbols (protein strings).
 """
 import ctypes as C
 
@@ -70,6 +71,8 @@ def global_align(pystr_seqj, pystr_seqi, matrix, gap_incentive, gap_open=-1, gap
     if codes.max() >= matrix.shape[0] or max(cols) >= matrix.shape[1]:
         raise ValueError("sequence symbol outside the substitution matrix")
     rows = np.ascontiguousarray(matrix[codes][:, cols].T, dtype=np.int64)
+    if len(alphabet) > 8:
+        return _protein_align(engine, pystr_seqj, pystr_seqi, alphabet, rows, gi, gap_open, gap_extend)
     out_j = C.create_string_buffer(I + J + 1)
     out_i = C.create_string_buffer(I + J + 1)
     n, m = C.c_int32(0), C.c_int32(0)
@@ -81,3 +84,34 @@ def global_align(pystr_seqj, pystr_seqi, matrix, gap_incentive, gap_open=-1, gap
         raise EngineError("c2b_global_align failed (%d): %s" % (rc, engine.L.c2b_last_error(engine.h).decode()))
     s1, s2 = out_j.raw[:n.value].decode(), out_i.raw[:n.value].decode()
     return s1, s2, round(100 * m.value / float(n.value), 3)
+
+
+def spell(ops, n, read, ref):
+    """the aligned strings of an op stream of n columns (column k from the right: bits 2 (k & 31) of ops[k >> 5]; 0 both,
+    1 gap in the read, 2 gap in the reference)"""
+    a, b = [], []
+    j, i = len(read), len(ref)
+    for k in range(n):
+        op = (int(ops[k >> 5]) >> (2 * (k & 31))) & 3
+        if op != 1:
+            j -= 1
+        if op != 2:
+            i -= 1
+        a.append("-" if op == 1 else read[j])
+        b.append("-" if op == 2 else ref[i])
+    return "".join(reversed(a)), "".join(reversed(b))
+
+
+def _protein_align(engine, seqj, seqi, alphabet, rows, gi, gap_open, gap_extend):
+    """one read of 9-32 distinct symbols through c2b_protein_align; the engine's configuration is left as it is"""
+    from .engine import EngineError
+    ops = np.zeros(32, dtype=np.uint64)
+    n, m = np.zeros(1, dtype=np.int32), np.zeros(1, dtype=np.int32)
+    off = np.array([0, len(seqj)], dtype=np.int64)
+    rc = engine.L.c2b_protein_align(engine.h, seqi.encode(), len(seqi), seqj.encode(), off.ctypes.data, 1, alphabet.encode(),
+                                    len(alphabet), rows.ctypes.data, gi.ctypes.data, int(gap_open), int(gap_extend),
+                                    ops.ctypes.data, n.ctypes.data, m.ctypes.data)
+    if rc != 0:
+        raise EngineError("c2b_protein_align failed (%d): %s" % (rc, engine.L.c2b_last_error(engine.h).decode()))
+    s1, s2 = spell(ops, int(n[0]), seqj, seqi)
+    return s1, s2, round(100 * int(m[0]) / float(n[0]), 3)

@@ -19,6 +19,8 @@
 #include <cstring>
 #include <string>
 #include <thread>
+#include <memory>
+#include <unordered_map>
 #include <vector>
 
 #include "c2b_core.cuh"
@@ -26,6 +28,7 @@
 #include "c2b_annotate.cuh"
 #include "c2b_vcf.cuh"
 #include "c2b_base_edit.cuh"
+#include "c2b_amino.cuh"
 #include "c2b_fastq_int.h"
 
 using namespace c2b;
@@ -264,6 +267,7 @@ struct c2b_engine {
     // scratch
     DevBuf tb, tbb, tbq, bnd, ops, rgo, work, lut;
     DevBuf gops, gmeta, left, left2, left0, left1;   // device-pointer API: op streams / meta words / left-over lists of the last launch
+    DevBuf pro_tab, pro_in, pro_out, pro_tb, pro_bnd;  // protein alignment (c2b_protein_align): tables, reads, op streams, slabs
     int n_warps = 0, grid = 0, stage_cap = 0;
     int grid_a = 0, grid_b = 0, stage_cap_a = 0;       // ALIGN / CLASSIFY kernels
     int split_ok = 0, split_all = 0;                   // configuration admits the two-kernel form (some / all references)
@@ -427,7 +431,8 @@ int c2b_create(int device, c2b_engine **out)
 void c2b_destroy(c2b_engine *e)
 {
     if (!e) return;
-    DevBuf *bufs[] = {&e->tb, &e->tbb, &e->tbq, &e->bnd, &e->ops, &e->rgo, &e->work, &e->lut, &e->gops, &e->gmeta, &e->left, &e->left2, &e->left0, &e->left1};
+    DevBuf *bufs[] = {&e->tb, &e->tbb, &e->tbq, &e->bnd, &e->ops, &e->rgo, &e->work, &e->lut, &e->gops, &e->gmeta, &e->left, &e->left2, &e->left0, &e->left1,
+                      &e->pro_tab, &e->pro_in, &e->pro_out, &e->pro_tb, &e->pro_bnd};
     for (DevBuf *b : bufs) if (b->p) rt_free(b->p);
     for (auto &st : e->stage) {
         DevBuf *sb[] = {&st.reads, &st.off, &st.cnt, &st.qw, &st.rid, &st.recs, &st.alns, &st.str, &st.ed, &st.maxlen, &st.ord, &st.gops, &st.gmeta, &st.left, &st.left2, &st.left0, &st.left1};
@@ -771,16 +776,17 @@ static int ensure_scratch(c2b_engine *e, int maxJ)
 // holds a path score from the origin or from a min_score border (gap_open * I * J).  On the way there are at most min(I, J)
 // substitutions and I + J gap columns, each with one gap_open or gap_extend term; an inserted read base adds its row's
 // incentive (at most J of them), an opened deletion that of the row it leaves (distinct rows), a border cell gap_incentive[0].
+static bool score_fits(int64_t gap_open, int64_t gap_extend, int64_t I, int64_t maxJ, const RefHost &h)
+{
+    const int64_t go = std::abs(gap_open), gap = std::max(go, std::abs(gap_extend)), J = std::max<int64_t>(maxJ, 1);
+    const int64_t bound = go * I * J + std::min(I, J) * h.sabs + (I + J) * gap + J * h.gabs + h.gsum_abs + h.gi0_abs;
+    return 4 * bound + 3 <= (int64_t)INT32_MAX;
+}
 static int score_range_ok(c2b_engine *e, int64_t maxJ, const char *who)
 {
-    const int64_t go = std::abs((int64_t)e->prm.gap_open), gap = std::max(go, std::abs((int64_t)e->prm.gap_extend));
-    for (int r = 0; r < e->n_refs; r++) {
-        const RefHost &h = e->refs[r];
-        const int64_t I = (int64_t)h.seq.size(), J = std::max<int64_t>(maxJ, 1);
-        const int64_t bound = go * I * J + std::min(I, J) * h.sabs + (I + J) * gap + J * h.gabs + h.gsum_abs + h.gi0_abs;
-        if (4 * bound + 3 > (int64_t)INT32_MAX)
+    for (int r = 0; r < e->n_refs; r++)
+        if (!score_fits(e->prm.gap_open, e->prm.gap_extend, (int64_t)e->refs[r].seq.size(), maxJ, e->refs[r]))
             return fail(e, C2B_E_LIMIT, std::string(who) + ": scores, gap penalties and incentives can exceed the int32 range of the DP");
-    }
     return C2B_OK;
 }
 
@@ -2253,6 +2259,382 @@ int c2b_be_quilt_timings(const c2b_be_quilt *q, double *device_ms, double *group
 {
     if (!q || !device_ms || !group_ms) return C2B_E_ARG;
     *device_ms = q->device_ms; *group_ms = q->group_ms;
+    return C2B_OK;
+}
+
+}  // extern "C"
+
+// ----------------------------------------------------------------------------------------- protein alignment
+// The reference protein's tables in the layout of c2b_configure (RefDev: prof [nq][Ipad] = 4 * score, cIe, g4), uploaded to
+// e->pro_tab.  `rows` is [nq][I] = matrix[ord(ref[i])][ord(alphabet[q])].
+static int protein_ref(c2b_engine *e, const char *who, int I, int nq, const int64_t *rows, const int64_t *gi, int gap_extend, RefDev &d,
+                       RefHost &h)
+{
+    const int nrb = (I + 255) / 256, Ipad = nrb * 256;
+    memset(&d, 0, sizeof d);
+    d.I = I; d.nrb = nrb; d.Ipad = Ipad; d.kstar = (I - 1) & 7; d.lstar = ((I - 1) >> 3) & 31;
+    d.gi0_4 = (int32_t)(4 * gi[0]);
+    const int64_t lim = (1ll << 27);
+    h.sabs = h.gabs = h.gsum_abs = 0; h.gi0_abs = std::abs(gi[0]);
+    for (size_t k = 0; k < (size_t)nq * I; k++) {
+        if (rows[k] > lim || rows[k] < -lim) return fail(e, C2B_E_LIMIT, std::string(who) + ": substitution score out of range");
+        h.sabs = std::max<int64_t>(h.sabs, std::abs(rows[k]));
+    }
+    for (int i = 0; i <= I; i++) {
+        if (gi[i] > lim || gi[i] < -lim) return fail(e, C2B_E_LIMIT, std::string(who) + ": gap incentive out of range");
+        h.gabs = std::max<int64_t>(h.gabs, std::abs(gi[i])); h.gsum_abs += std::abs(gi[i]);
+    }
+    std::vector<int32_t> blob((size_t)(nq + 2) * Ipad, 0);
+    int32_t *prof = blob.data(), *cIe = prof + (size_t)nq * Ipad, *g4 = cIe + Ipad;
+    for (int q = 0; q < nq; q++)
+        for (int i = 0; i < I; i++) prof[(size_t)q * Ipad + i] = (int32_t)(4 * rows[(size_t)q * I + i]);
+    for (int i = 0; i < I; i++) { cIe[i] = (int32_t)(4 * (gap_extend + gi[i + 1])); g4[i] = (int32_t)(4 * gi[i]); }
+    int rc;
+    if ((rc = ensure(e, e->pro_tab, blob.size() * 4))) return rc;
+    RTCHK(rt_h2d(e->pro_tab.p, blob.data(), blob.size() * 4, e->stream));
+    const int32_t *dp = (const int32_t *)e->pro_tab.p;
+    d.prof = dp; d.cIe = dp + (size_t)nq * Ipad; d.g4 = d.cIe + Ipad;
+    return C2B_OK;
+}
+
+// global_align of n reads (alphabet codes codes[off[r] .. off[r+1])) against one reference protein: ops [n][32] (column k from
+// the right: bits 2 (k & 31) of word k >> 5), nops[n] = alignment columns.  Limits first, nothing launched past one.
+static int protein_batch(c2b_engine *e, const char *who, int I, int nq, const int64_t *rows, const int64_t *gi, int go, int ge,
+                         const uint8_t *codes, const int64_t *off, int64_t n, uint64_t *ops, int32_t *nops, int64_t *bad = nullptr)
+{
+    if (I < 1 || I > C2B_MAX_REF_LEN) return fail(e, C2B_E_LIMIT, std::string(who) + ": reference empty or longer than C2B_MAX_REF_LEN");
+    if (nq < 1 || nq > C2B_AA_MAX_Q) return fail(e, C2B_E_LIMIT, std::string(who) + ": alphabet larger than C2B_AA_MAX_Q");
+    int64_t maxJ = 0;
+    for (int64_t r = 0; r < n; r++) {
+        const int64_t J = off[r + 1] - off[r];
+        if (J < 1 || J > C2B_MAX_READ_LEN || I + J > C2B_MAX_ALN_LEN)
+            return fail(e, C2B_E_LIMIT, std::string(who) + ": read " + std::to_string(r) + " empty or beyond C2B_MAX_READ_LEN / C2B_MAX_ALN_LEN");
+        maxJ = std::max(maxJ, J);
+    }
+    for (int64_t k = 0; k < off[n]; k++)
+        if (codes[k] >= nq) return fail(e, C2B_E_ARG, std::string(who) + ": read symbol outside the alphabet");
+    RefDev d; RefHost h;
+    int rc;
+    if ((rc = protein_ref(e, who, I, nq, rows, gi, ge, d, h))) return rc;
+    if (!score_fits(go, ge, I, maxJ, h))
+        return fail(e, C2B_E_LIMIT, std::string(who) + ": scores, gap penalties and incentives can exceed the int32 range of the DP");
+    if (n == 0) return C2B_OK;
+    const int TS = (int)((maxJ + 32 + 31) & ~31);
+    const int64_t nw = std::min<int64_t>(n, std::max(e->n_warps, 1));
+    aa::PParams P;
+    memset(&P, 0, sizeof P);
+    P.K.go = go; P.K.ge = ge; P.K.TS = TS;
+    P.K.tb_words_per_warp = (int64_t)d.nrb * TS * 32; P.K.bnd_words_per_warp = 2 * 3 * (int64_t)TS;
+    if ((rc = ensure(e, e->pro_tb, (size_t)(nw * P.K.tb_words_per_warp * 4)))) return rc;
+    if ((rc = ensure(e, e->pro_bnd, (size_t)(nw * P.K.bnd_words_per_warp * 4)))) return rc;
+    const size_t o_off = ChunkPipe::al((size_t)off[n]), in_end = o_off + (size_t)(n + 1) * 8;
+    const size_t o_n = (size_t)n * 32 * 8, out_end = o_n + (size_t)n * 4;
+    if ((rc = ensure(e, e->pro_in, in_end))) return rc;
+    if ((rc = ensure(e, e->pro_out, out_end))) return rc;
+    RTCHK(rt_h2d(e->pro_in.p, codes, (size_t)off[n], e->stream));
+    RTCHK(rt_h2d((char *)e->pro_in.p + o_off, off, (size_t)(n + 1) * 8, e->stream));
+    P.K.tb = (uint32_t *)e->pro_tb.p; P.K.bnd = (int32_t *)e->pro_bnd.p;
+    P.R = d;
+    P.codes = (const uint8_t *)e->pro_in.p; P.off = (const int64_t *)((const char *)e->pro_in.p + o_off); P.n = n;
+    P.ops = (uint64_t *)e->pro_out.p; P.nops = (int32_t *)((char *)e->pro_out.p + o_n);
+#ifndef C2B_EMU
+    c2b_protein_kernel<<<(int)((nw + 7) / 8), 256, 0, e->stream>>>(P);
+    RTCHK(cudaGetLastError());
+#else
+    for (int64_t r = 0; r < n; r++) emu::run_warp([&]() { aa::protein_one(P, r, 0); });
+#endif
+    RTCHK(rt_d2h(ops, P.ops, o_n, e->stream));
+    RTCHK(rt_d2h(nops, P.nops, (size_t)n * 4, e->stream));
+    RTCHK(rt_sync(e->stream));
+    for (int64_t r = 0; r < n; r++)
+        if (nops[r] < 0) {
+            if (bad) *bad = r;
+            return fail(e, C2B_E_STATE, std::string(who) + ": the traceback of read " + std::to_string(r) +
+                                            " leaves the zone where global_align is defined (SURVEY 3.2)");
+        }
+    return C2B_OK;
+}
+
+// the aligned strings of one op stream (right to left), written left-justified to out_read / out_ref -> matched columns
+static int32_t spell_ops(const uint64_t *ops, int32_t n, const uint8_t *read, int64_t J, const uint8_t *ref, int64_t I, uint8_t *out_read,
+                         uint8_t *out_ref)
+{
+    int64_t j = J, i = I;
+    int32_t m = 0;
+    for (int32_t k = 0, c = n - 1; k < n; k++, c--) {
+        const int op = (int)((ops[k >> 5] >> (2 * (k & 31))) & 3u);
+        const uint8_t a = op == OP_J ? '-' : read[--j], b = op == OP_I ? '-' : ref[--i];
+        out_read[c] = a; out_ref[c] = b;
+        m += op == OP_M && a == b;
+    }
+    return m;
+}
+
+// --coding_seq amino-acid table: every row's aligned strings (arena) and the sorted groups, whose strings point into it
+struct c2b_amino {
+    std::vector<uint8_t> arena;
+    std::vector<c2b_cut_group> groups;
+    std::vector<int64_t> ref_len;                              // per row: residues of the reference protein
+    int64_t n_pairs = 0;
+    double row_ms = 0, align_ms = 0, group_ms = 0;
+};
+
+// the standard genetic code, codon index 16 a + 4 b + c over A C G T (CRISPRessoShared.CODON_TO_AMINO_ACID_SINGLE_CHAR)
+static const char AA_TABLE[65] = "KNKNTTTTRSRSIIMIQHQHPPPPRRRRLLLLEDEDAAAAGGGGVVVV*Y*YSSSS*CWCLFLF";
+
+extern "C" {
+
+int c2b_protein_align(c2b_engine *e, const char *ref, int32_t ref_len, const char *reads, const int64_t *offsets, int64_t n,
+                      const char *alphabet, int32_t nq, const int64_t *score_rows, const int64_t *gap_incentive, int32_t gap_open,
+                      int32_t gap_extend, uint64_t *ops, int32_t *aln_len, int32_t *n_match)
+{
+    if (!e || !ref || !offsets || n < 0 || !alphabet || !score_rows || !gap_incentive || (n && (!ops || !aln_len || !n_match)) ||
+        (n && offsets[n] && !reads))
+        return fail(e, C2B_E_ARG, "c2b_protein_align: bad argument");
+    const int64_t *offs[1] = {offsets};
+    if (!offsets_ok(offs, 1, n)) return fail(e, C2B_E_ARG, "c2b_protein_align: offsets must start at 0 and not decrease");
+    if (nq < 1 || nq > C2B_AA_MAX_Q) return fail(e, C2B_E_LIMIT, "c2b_protein_align: alphabet larger than C2B_AA_MAX_Q");
+    uint8_t lut[256];
+    memset(lut, 255, sizeof lut);
+    for (int q = 0; q < nq; q++) lut[(uint8_t)alphabet[q]] = (uint8_t)q;
+    std::vector<uint8_t> codes((size_t)offsets[n]);
+    for (int64_t k = 0; k < offsets[n]; k++) codes[(size_t)k] = lut[(uint8_t)reads[k]];
+    int rc = protein_batch(e, "c2b_protein_align", ref_len, nq, score_rows, gap_incentive, gap_open, gap_extend, codes.data(), offsets, n,
+                           ops, aln_len);
+    if (rc) return rc;
+    std::vector<uint8_t> a((size_t)C2B_MAX_ALN_LEN), b((size_t)C2B_MAX_ALN_LEN);
+    for (int64_t r = 0; r < n; r++)
+        n_match[r] = spell_ops(ops + r * 32, aln_len[r], (const uint8_t *)reads + offsets[r], offsets[r + 1] - offsets[r],
+                               (const uint8_t *)ref, ref_len, a.data(), b.data());
+    return C2B_OK;
+}
+
+// get_amino_acid_dataframe over packed allele rows: the row pass in chunks (ChunkPipe, c2b_amino.cuh), one global_align per
+// distinct (read protein, reference protein) pair (c2b_vcf_sum_records' exact hash; one protein_batch per reference protein),
+// silent edits and truncation per row on host threads, then c2b_group_around_cut.
+int c2b_amino_table(c2b_engine *e, int64_t n_rows, int64_t plot_left_idx, const uint8_t *ref, const int64_t *ref_off, const uint8_t *aln,
+                    const int64_t *aln_off, const int64_t *rp, const int64_t *rp_off, const int64_t *matrix, int32_t msize,
+                    int64_t cut_point, int64_t seq_len, const uint8_t *unedited, const int64_t *n_deleted, const int64_t *n_inserted,
+                    const int64_t *n_mutated, const int64_t *reads, const double *pct, int64_t chunk, int64_t *err, c2b_amino **out)
+{
+    if (!e || !out || !err || n_rows < 0 || !ref_off || !aln_off || !rp_off || !matrix || msize < 1)
+        return fail(e, C2B_E_ARG, "c2b_amino_table: bad argument");
+    *out = nullptr;
+    err[0] = -1; err[1] = 0;
+    const int64_t *offs[3] = {ref_off, aln_off, rp_off};
+    if (!offsets_ok(offs, 3, n_rows)) return fail(e, C2B_E_ARG, "c2b_amino_table: offsets must start at 0 and not decrease");
+    if (n_rows && (!unedited || !n_deleted || !n_inserted || !n_mutated || !reads || !pct || (ref_off[n_rows] && !ref) ||
+                   (aln_off[n_rows] && !aln) || (rp_off[n_rows] && !rp)))
+        return fail(e, C2B_E_ARG, "c2b_amino_table: row arrays missing");
+    if (chunk <= 0) chunk = 1 << 14;
+    const auto t0 = std::chrono::steady_clock::now();
+    std::unique_ptr<c2b_amino> A(new c2b_amino());
+    A->ref_len.assign((size_t)n_rows, 0);
+    // per row: key = read protein | 0 | reference protein, and at the same offsets the codon indices
+    std::vector<uint8_t> key, cod;
+    std::vector<int64_t> koff(1, 0), na((size_t)n_rows);
+    const RowCol cols[3] = {{ref, ref_off, 1}, {aln, aln_off, 1}, {rp, rp_off, 8}};
+    int rc = C2B_OK;
+    {
+        ChunkPipe cp(e);
+        auto al = ChunkPipe::al;
+        const char *dt = nullptr;
+        rc = cp.fixed(AA_TABLE, 64, &dt);
+        for (int64_t r0 = 0; !rc && r0 < n_rows; r0 += chunk) {
+            const int64_t r1 = std::min(n_rows, r0 + chunk), m = r1 - r0;
+            const int64_t ab = aln_off[r1] - aln_off[r0], fb = ref_off[r1] - ref_off[r0];
+            const char *d[3]; const int64_t *o[3];
+            if ((rc = cp.upload(cols, 3, r0, r1, d, o))) break;
+            // out: read protein | read codons (at aln offsets) | reference protein | reference codons (at ref offsets) | len | err
+            const size_t o_rc = al((size_t)ab), o_fa = o_rc + al((size_t)ab), o_fc = o_fa + al((size_t)fb), o_len = o_fc + al((size_t)fb),
+                         o_err = o_len + al((size_t)m * 16), o_end = o_err + (size_t)m * 8;
+            if ((rc = ensure(e, cp.d_out, o_end + 16))) break;
+            char *dout = (char *)cp.d_out.p;
+            aa::RParams P;
+            memset(&P, 0, sizeof P);
+            P.n = m; P.left = plot_left_idx; P.table = (const uint8_t *)dt;
+            P.ref = (const uint8_t *)d[0]; P.ref_off = o[0]; P.aln = (const uint8_t *)d[1]; P.aln_off = o[1];
+            P.rp = (const int64_t *)d[2]; P.rp_off = o[2];
+            P.raa = (uint8_t *)dout; P.rcod = (uint8_t *)dout + o_rc; P.faa = (uint8_t *)dout + o_fa; P.fcod = (uint8_t *)dout + o_fc;
+            P.len = (int64_t *)(dout + o_len); P.err = (int64_t *)(dout + o_err);
+#ifndef C2B_EMU
+            c2b_amino_codons_kernel<<<row_grid(m), 256, 0, e->stream>>>(P);
+            if (cudaGetLastError() != cudaSuccess) { rc = fail(e, C2B_E_CUDA, "c2b_amino_table: launch failed"); break; }
+#else
+            for (int64_t r = 0; r < m; r++) emu::run_warp([&]() { aa::codons_one(P, r); });
+#endif
+            const uint8_t *h;
+            if ((rc = cp.download(o_end, &h))) break;
+            const int64_t *hl = (const int64_t *)(h + o_len), *he = (const int64_t *)(h + o_err);
+            for (int64_t r = 0; r < m && err[0] < 0; r++)
+                if (he[r]) { err[0] = r0 + r; err[1] = he[r]; }
+            if (err[0] >= 0) break;
+            for (int64_t r = 0; r < m; r++) {
+                const int64_t a0 = aln_off[r0 + r] - aln_off[r0], f0 = ref_off[r0 + r] - ref_off[r0], a = hl[2 * r], f = hl[2 * r + 1];
+                na[(size_t)(r0 + r)] = a;
+                A->ref_len[(size_t)(r0 + r)] = f;
+                key.insert(key.end(), h + a0, h + a0 + a); key.push_back(0); key.insert(key.end(), h + o_fa + f0, h + o_fa + f0 + f);
+                cod.insert(cod.end(), h + o_rc + a0, h + o_rc + a0 + a); cod.push_back(0);
+                cod.insert(cod.end(), h + o_fc + f0, h + o_fc + f0 + f);
+                koff.push_back((int64_t)key.size());
+            }
+        }
+    }
+    if (rc) return rc;
+    if (err[0] >= 0) {
+        static const char *what[4] = {"", "ValueError: plot_left_idx is not in ref_positions", "KeyError: a codon outside the table",
+                                      "a translation shorter than one codon (global_align is undefined on an empty sequence)"};
+        char msg[200];
+        snprintf(msg, sizeof msg, "c2b_amino_table: row %lld raises %s", (long long)err[0], what[err[1] >= 1 && err[1] <= 3 ? err[1] : 0]);
+        return fail(e, C2B_E_ARG, msg);
+    }
+    const auto t1 = std::chrono::steady_clock::now();
+    // distinct pairs, first-seen order; one batch per distinct reference protein
+    c2b_vcf_counts U;
+    std::vector<int64_t> uix((size_t)n_rows);
+    c2b_vcf_sum_records(key.data(), koff.data(), nullptr, n_rows, &U, uix.data());
+    const int64_t nu = (int64_t)U.key_off.size() - 1;
+    A->n_pairs = nu;
+    const uint8_t *uk = U.keys.get();
+    std::vector<int64_t> ualn_off((size_t)nu + 1, 0), ucols((size_t)nu);
+    std::vector<uint8_t> ualn;                               // per pair: aligned read | aligned reference
+    {
+        std::vector<std::pair<std::string, std::vector<int64_t>>> by_ref;
+        std::unordered_map<std::string, size_t> ref_at;
+        std::vector<int64_t> sep((size_t)nu);
+        for (int64_t u = 0; u < nu; u++) {
+            const uint8_t *p = uk + U.key_off[(size_t)u];
+            const int64_t len = U.key_off[(size_t)u + 1] - U.key_off[(size_t)u];
+            sep[(size_t)u] = (int64_t)((const uint8_t *)memchr(p, 0, (size_t)len) - p);
+            std::string f((const char *)p + sep[(size_t)u] + 1, (size_t)(len - sep[(size_t)u] - 1));
+            auto it = ref_at.find(f);
+            if (it == ref_at.end()) { it = ref_at.emplace(f, by_ref.size()).first; by_ref.push_back({f, {}}); }
+            by_ref[it->second].second.push_back(u);
+        }
+        std::vector<std::vector<uint64_t>> uops((size_t)nu);
+        std::vector<int32_t> un((size_t)nu);
+        for (auto &br : by_ref) {
+            const std::string &f = br.first;
+            const std::vector<int64_t> &us = br.second;
+            const int I = (int)std::min<size_t>(f.size(), (size_t)C2B_MAX_REF_LEN + 1);
+            bool seen[256] = {false};
+            for (int64_t u : us) for (int64_t x = 0; x < sep[(size_t)u]; x++) seen[uk[U.key_off[(size_t)u] + x]] = true;
+            std::string alpha;
+            for (int c = 0; c < 256; c++) if (seen[c]) alpha.push_back((char)c);
+            const int nq = (int)alpha.size();
+            if (nq > C2B_AA_MAX_Q) return fail(e, C2B_E_LIMIT, "c2b_amino_table: read alphabet larger than C2B_AA_MAX_Q");
+            for (char c : alpha + f)
+                if ((uint8_t)c >= (uint32_t)msize) return fail(e, C2B_E_ARG, "c2b_amino_table: amino acid outside the substitution matrix");
+            std::vector<int64_t> rows((size_t)nq * I), gi((size_t)I + 1, 0);
+            for (int q = 0; q < nq; q++)
+                for (int i = 0; i < I; i++) rows[(size_t)q * I + i] = matrix[(size_t)(uint8_t)f[(size_t)i] * msize + (uint8_t)alpha[(size_t)q]];
+            if (cut_point >= 0 && cut_point <= I) gi[(size_t)cut_point] = 1;
+            uint8_t lut[256];
+            for (int q = 0; q < nq; q++) lut[(uint8_t)alpha[(size_t)q]] = (uint8_t)q;
+            std::vector<uint8_t> codes;
+            std::vector<int64_t> off(1, 0);
+            for (int64_t u : us) {
+                for (int64_t x = 0; x < sep[(size_t)u]; x++) codes.push_back(lut[uk[U.key_off[(size_t)u] + x]]);
+                off.push_back((int64_t)codes.size());
+            }
+            const int64_t nb = (int64_t)us.size();
+            std::vector<uint64_t> ops((size_t)nb * 32);
+            std::vector<int32_t> nops((size_t)nb);
+            int64_t bad = -1;
+            if ((rc = protein_batch(e, "c2b_amino_table", I, nq, rows.data(), gi.data(), -1, -1, codes.data(), off.data(), nb, ops.data(),
+                                    nops.data(), &bad))) {
+                if (bad < 0) return rc;
+                for (int64_t r = 0; r < n_rows && err[0] < 0; r++) if (uix[(size_t)r] == us[(size_t)bad]) err[0] = r;
+                err[1] = aa::E_UNDEFINED;
+                return fail(e, C2B_E_ARG, "c2b_amino_table: row " + std::to_string(err[0]) +
+                                              ": global_align's traceback leaves the zone where it is defined (SURVEY 3.2)");
+            }
+            for (int64_t k = 0; k < nb; k++) {
+                uops[(size_t)us[(size_t)k]].assign(ops.begin() + k * 32, ops.begin() + k * 32 + 32);
+                un[(size_t)us[(size_t)k]] = nops[(size_t)k];
+            }
+        }
+        for (int64_t u = 0; u < nu; u++) { ucols[(size_t)u] = un[(size_t)u]; ualn_off[(size_t)u + 1] = ualn_off[(size_t)u] + 2 * un[(size_t)u]; }
+        ualn.resize((size_t)ualn_off[(size_t)nu]);
+        for (int64_t u = 0; u < nu; u++) {
+            const uint8_t *p = uk + U.key_off[(size_t)u];
+            const int64_t s = sep[(size_t)u], len = U.key_off[(size_t)u + 1] - U.key_off[(size_t)u];
+            uint8_t *o = ualn.data() + ualn_off[(size_t)u];
+            spell_ops(uops[(size_t)u].data(), un[(size_t)u], p, s, p + s + 1, len - s - 1, o, o + un[(size_t)u]);
+        }
+    }
+    const auto t2 = std::chrono::steady_clock::now();
+    // per row: get_silent_edits (a read residue equal to the reference's but from another codon is lower-cased), then
+    // [:sequence_length] with Python's slice bounds
+    std::vector<int64_t> roff((size_t)n_rows + 1, 0);
+    auto cut_len = [&](int64_t n) { int64_t k = seq_len < 0 ? std::max<int64_t>(0, n + seq_len) : seq_len; return std::min(k, n); };
+    for (int64_t r = 0; r < n_rows; r++) roff[(size_t)r + 1] = roff[(size_t)r] + 2 * cut_len(ucols[(size_t)uix[(size_t)r]]);
+    A->arena.resize((size_t)roff[(size_t)n_rows] + 1);
+    std::vector<c2b_cut_group> rows((size_t)n_rows);
+    {
+        const int T = (int)std::max<int64_t>(1, std::min<int64_t>({(int64_t)std::thread::hardware_concurrency(), 32, n_rows / 4096 + 1}));
+        auto work = [&](int t) {
+            for (int64_t r = n_rows * t / T; r < n_rows * (t + 1) / T; r++) {
+                const int64_t u = uix[(size_t)r], n = ucols[(size_t)u], L = cut_len(n);
+                const uint8_t *sa = ualn.data() + ualn_off[(size_t)u], *sb = sa + n;
+                const uint8_t *rc_ = cod.data() + koff[(size_t)r], *fc = rc_ + na[(size_t)r] + 1;
+                uint8_t *o = A->arena.data() + roff[(size_t)r];
+                int64_t x = 0, y = 0;
+                for (int64_t c = 0; c < n; c++) {
+                    const bool ga = sa[c] == '-', gb = sb[c] == '-';
+                    if (c < L) { o[c] = (!ga && !gb && sa[c] == sb[c] && rc_[x] != fc[y]) ? (uint8_t)tolower(sa[c]) : sa[c]; o[L + c] = sb[c]; }
+                    x += !ga; y += !gb;
+                }
+                c2b_cut_group &G = rows[(size_t)r];
+                G.seq = o; G.ref = o + L; G.len = L;
+                G.unedited = unedited[r] ? 1 : 0; G.ndel = n_deleted[r]; G.nins = n_inserted[r]; G.nmut = n_mutated[r];
+                G.reads = reads[r]; G.pct = pct[r];
+            }
+        };
+        std::vector<std::thread> th;
+        for (int t = 1; t < T; t++) th.emplace_back(work, t);
+        work(0);
+        for (auto &x : th) x.join();
+    }
+    A->groups = c2b_group_around_cut(rows);
+    const auto t3 = std::chrono::steady_clock::now();
+    A->row_ms = std::chrono::duration<double, std::milli>(t1 - t0).count();
+    A->align_ms = std::chrono::duration<double, std::milli>(t2 - t1).count();
+    A->group_ms = std::chrono::duration<double, std::milli>(t3 - t2).count();
+    *out = A.release();
+    return C2B_OK;
+}
+
+void c2b_amino_free(c2b_amino *a) { delete a; }
+int64_t c2b_amino_n(const c2b_amino *a) { return a ? (int64_t)a->groups.size() : 0; }
+int64_t c2b_amino_bytes(const c2b_amino *a)
+{
+    int64_t n = 0;
+    if (a) for (const c2b_cut_group &G : a->groups) n += G.len;
+    return n;
+}
+const int64_t *c2b_amino_ref_lens(const c2b_amino *a) { return a && !a->ref_len.empty() ? a->ref_len.data() : nullptr; }
+int c2b_amino_fetch(const c2b_amino *a, uint8_t *seq, uint8_t *ref, int64_t *seq_off, uint8_t *unedited, int64_t *n_deleted,
+                    int64_t *n_inserted, int64_t *n_mutated, int64_t *reads, double *pct)
+{
+    if (!a || !seq_off || !unedited || !n_deleted || !n_inserted || !n_mutated || !reads || !pct) return C2B_E_ARG;
+    int64_t o = 0;
+    seq_off[0] = 0;
+    for (size_t g = 0; g < a->groups.size(); g++) {
+        const c2b_cut_group &G = a->groups[g];
+        if (G.len) {
+            if (!seq || !ref) return C2B_E_ARG;
+            memcpy(seq + o, G.seq, (size_t)G.len); memcpy(ref + o, G.ref, (size_t)G.len);
+        }
+        o += G.len; seq_off[g + 1] = o;
+        unedited[g] = G.unedited; n_deleted[g] = G.ndel; n_inserted[g] = G.nins; n_mutated[g] = G.nmut; reads[g] = G.reads; pct[g] = G.pct;
+    }
+    return C2B_OK;
+}
+int c2b_amino_timings(const c2b_amino *a, double *row_ms, double *align_ms, double *group_ms, int64_t *n_pairs)
+{
+    if (!a || !row_ms || !align_ms || !group_ms || !n_pairs) return C2B_E_ARG;
+    *row_ms = a->row_ms; *align_ms = a->align_ms; *group_ms = a->group_ms; *n_pairs = a->n_pairs;
     return C2B_OK;
 }
 

@@ -225,8 +225,9 @@ bool read_gz(const char *path, c2b_bytes &buf, std::string &err)
 // `weight`, each unique's sum of its records' weights goes to sums[u]; *overflow is set when one leaves int64)
 void dedup_records(const std::vector<Seq> &seq, const std::vector<uint64_t> &hv, int64_t n_rec, int T, c2b_fastq *F,
                    const std::function<void(const char *)> &lap, const int64_t *weight = nullptr,
-                   std::vector<int64_t> *sums = nullptr, std::atomic<bool> *overflow = nullptr)
+                   std::vector<int64_t> *sums = nullptr, std::atomic<bool> *overflow = nullptr, int64_t *index = nullptr)
 {
+    // index (optional): index[r] = the number of record r's unique, via the first record of its unique while deduplicating
     // (3) sharded exact dedup in file order
     struct Ent { int64_t first; int32_t count; int64_t sum; };
     std::vector<std::vector<Ent>> found(T);
@@ -243,10 +244,11 @@ void dedup_records(const std::vector<Seq> &seq, const std::vector<uint64_t> &hv,
             size_t k = (size_t)h & (cap - 1);
             for (;;) {
                 const int32_t e = slot[k];
-                if (e < 0) { slot[k] = (int32_t)E.size(); E.push_back({r, 1, weight ? weight[r] : 0}); break; }
+                if (e < 0) { slot[k] = (int32_t)E.size(); E.push_back({r, 1, weight ? weight[r] : 0}); if (index) index[r] = r; break; }
                 const Seq &a = seq[(size_t)E[(size_t)e].first], &b = seq[(size_t)r];
                 if (hv[(size_t)E[(size_t)e].first] == h && a.len == b.len && memcmp(a.p, b.p, a.len) == 0) {
                     E[(size_t)e].count++;
+                    if (index) index[r] = E[(size_t)e].first;
                     if (weight && __builtin_add_overflow(E[(size_t)e].sum, weight[r], &E[(size_t)e].sum)) overflow->store(true);
                     break;
                 }
@@ -299,6 +301,7 @@ void dedup_records(const std::vector<Seq> &seq, const std::vector<uint64_t> &hv,
     F->offsets[nu] = tot;
     F->seqs.reset(new uint8_t[(size_t)tot + 16]);
     if (weight) sums->resize(nu);
+    std::vector<int64_t> u_at(index ? (size_t)n_rec : 0);
     {
         auto emit = [&](int t) {
             size_t u = u0[(size_t)t]; int64_t by = b0[(size_t)t];
@@ -307,6 +310,7 @@ void dedup_records(const std::vector<Seq> &seq, const std::vector<uint64_t> &hv,
                 if (!c) continue;
                 const Seq &q = seq[(size_t)r];
                 F->offsets[u] = by; F->counts[u] = c; F->first_index[u] = r;
+                if (index) u_at[(size_t)r] = (int64_t)u;
                 if (weight) (*sums)[u] = sum_at[(size_t)r];
                 memcpy(F->seqs.get() + by, q.p, q.len);
                 by += q.len; u++;
@@ -317,12 +321,14 @@ void dedup_records(const std::vector<Seq> &seq, const std::vector<uint64_t> &hv,
         emit(0);
         for (auto &x : th) x.join();
     }
+    if (index)
+        run_threads(T, [&](int t) { for (int64_t r = rec_lo(t); r < rec_lo(t + 1); r++) index[r] = u_at[(size_t)index[r]]; });
     lap("emit");
 }
 
 }  // namespace
 
-bool c2b_vcf_sum_records(const uint8_t *arena, const int64_t *off, const int64_t *w, int64_t n, c2b_vcf_counts *out)
+bool c2b_vcf_sum_records(const uint8_t *arena, const int64_t *off, const int64_t *w, int64_t n, c2b_vcf_counts *out, int64_t *index)
 {
     std::vector<Seq> seq((size_t)n);
     std::vector<uint64_t> hv((size_t)n);
@@ -335,7 +341,7 @@ bool c2b_vcf_sum_records(const uint8_t *arena, const int64_t *off, const int64_t
     });
     c2b_fastq F;
     std::atomic<bool> overflow(false);
-    dedup_records(seq, hv, n, T, &F, [](const char *) {}, w, &out->reads, &overflow);
+    dedup_records(seq, hv, n, T, &F, [](const char *) {}, w, w ? &out->reads : nullptr, &overflow, index);
     out->keys = std::move(F.seqs);
     out->key_off = std::move(F.offsets);
     out->n_records = n;

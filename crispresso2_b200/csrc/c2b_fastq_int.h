@@ -49,8 +49,9 @@ struct c2b_vcf_counts {
     double device_ms = 0, sum_ms = 0;
 };
 // the records rec[i] = arena[off[i] .. off[i+1]) with weights w[i], equal records summed (the exact hash of the FASTQ front end);
-// false when a sum leaves int64
-bool c2b_vcf_sum_records(const uint8_t *arena, const int64_t *off, const int64_t *w, int64_t n, c2b_vcf_counts *out);
+// false when a sum leaves int64.  w may be nullptr (no sums); index (optional): index[i] = the number of record i's key
+bool c2b_vcf_sum_records(const uint8_t *arena, const int64_t *off, const int64_t *w, int64_t n, c2b_vcf_counts *out,
+                         int64_t *index = nullptr);
 
 // One row, or one group, of the tables around the cut before pandas' groupby (get_dataframe_around_cut_asymmetrical,
 // get_base_edit_dataframe_around_cut): Aligned_Sequence seq[0 .. len) and Reference_Sequence ref[0 .. len), the other key columns,

@@ -24,6 +24,8 @@ What is re-bound (INTEGRATION.md section 2), nothing else of the reference chang
   * CRISPRessoShared.get_base_edit_dataframe_around_cut (called by data_prep.prep_base_edit_quilt, :1675)
     -> crispresso2_b200.base_edit.get_base_edit_dataframe_around_cut on the launcher's engine
     (--base_editor_output, figures 10i and 10h; both in single-process runs and under torchrun alike)
+  * CRISPRessoShared.get_amino_acid_dataframe (called by data_prep.prep_amino_acid_table, :1360; --coding_seq with plots on)
+    -> crispresso2_b200.amino_acids.get_amino_acid_dataframe on the launcher's engine (single process and torchrun alike)
 Under torchrun (WORLD_SIZE > 1) every rank runs the same command; process_fastq shards the unique reads over the ranks' GPUs
 and merges the count block with one all-reduce (core.process_fastq_sharded); rank 0's output directory is the result.
 
@@ -152,6 +154,15 @@ def bind(CORE=None, engine=None, lib_path=None):
     CORE.CRISPRessoPlotData.get_upset_plot_counts = get_upset_plot_counts
     CORE.get_upset_plot_counts = get_upset_plot_counts
     SH.get_base_edit_dataframe_around_cut = get_base_edit_dataframe_around_cut
+    # --coding_seq amino-acid tables: translations and protein alignments on the GPU, grouped natively (amino_acids.py)
+    from . import amino_acids
+
+    def get_amino_acid_dataframe(df_alleles, plot_left_idx, sequence_length, matrix_path, amino_acid_cut_point,
+                                 collapse_by_sequence=True):
+        return amino_acids.get_amino_acid_dataframe(df_alleles, plot_left_idx, sequence_length, matrix_path, amino_acid_cut_point,
+                                                    collapse_by_sequence, engine=get_engine())
+
+    SH.get_amino_acid_dataframe = get_amino_acid_dataframe
     return CORE
 
 

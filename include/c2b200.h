@@ -550,6 +550,47 @@ int  c2b_be_quilt_fetch(const c2b_be_quilt *q, uint8_t *seq, int64_t *seq_off, u
 /* wall time of the call's device pass with its copies, and of the host grouping, in ms */
 int  c2b_be_quilt_timings(const c2b_be_quilt *q, double *device_ms, double *group_ms);
 
+/* ---- --coding_seq amino-acid tables (csrc/c2b_amino.cuh, c2b_engine.cu) ----
+ * c2b_protein_align replaces: CRISPResso2Align.global_align (Align.pyx:101-434) of protein strings, as get_amino_acid_row calls it
+ * (CRISPRessoShared.py:1602-1607).  The n reads reads[offsets[r] .. offsets[r+1]) (symbols of `alphabet`, up to C2B_AA_MAX_Q of
+ * them) are each aligned to `ref` with the engine's 32-bit DP and traceback, forward strand, no seed test; score_rows is
+ * [nq][ref_len] = matrix[ord(ref[i])][ord(alphabet[q])], gap_incentive has ref_len + 1 entries.  Per read: its op stream
+ * ops[32 r .. 32 r + 31] (column k from the right in bits 2 (k & 31) of word k >> 5; 0 both, 1 gap in the read, 2 gap in the
+ * reference), its number of columns and of columns with equal symbols.  The engine's configuration is not touched.
+ * C2B_E_LIMIT, before any launch: a reference longer than C2B_MAX_REF_LEN, an empty read, a read longer than C2B_MAX_READ_LEN,
+ * ref_len + read length above C2B_MAX_ALN_LEN, a score or incentive beyond 2**27, or scores that can leave the DP's int32.      */
+#define C2B_AA_MAX_Q 32
+int  c2b_protein_align(c2b_engine *e, const char *ref, int32_t ref_len, const char *reads, const int64_t *offsets, int64_t n,
+                       const char *alphabet, int32_t nq, const int64_t *score_rows, const int64_t *gap_incentive, int32_t gap_open,
+                       int32_t gap_extend, uint64_t *ops, int32_t *aln_len, int32_t *n_match);
+
+/* c2b_amino replaces: get_amino_acid_dataframe with get_amino_acid_row (CRISPRessoShared.py:1557-1653) up to its groupby and sort.
+ * Per row: left_idx = ref_positions.index(plot_left_idx), the gap-stripped suffixes of Aligned_Sequence and Reference_Sequence
+ * from left_idx translated codon by codon (the standard code, CODON_TO_AMINO_ACID_SINGLE_CHAR), global_align of the two proteins
+ * under `matrix` (msize x msize, matrix[a * msize + b]) at gap_open = gap_extend = -1 with gap_incentive 1 at cut_point when
+ * 0 <= cut_point <= len(reference protein) -- once per distinct pair --, get_silent_edits (lower case where the residues are equal
+ * and the codons differ), both strings cut to [:seq_len], then the grouping and sort of c2b_be_quilt over the six key columns.
+ * When a row raises in the reference, returns C2B_E_ARG with err[0..1] = the first such row and C2B_AA_E_*; err[0] = -1
+ * otherwise.                                                                                                                  */
+#define C2B_AA_E_NOT_IN_LIST 1      /* ValueError: plot_left_idx is not in ref_positions */
+#define C2B_AA_E_CODON       2      /* KeyError: a codon outside the table (the read's first) */
+#define C2B_AA_E_EMPTY       3      /* a protein shorter than one residue: global_align is undefined there (refused) */
+#define C2B_AA_E_UNDEFINED   4      /* the row's traceback leaves the zone where global_align is defined (SURVEY 3.2; refused) */
+typedef struct c2b_amino c2b_amino;
+int  c2b_amino_table(c2b_engine *e, int64_t n_rows, int64_t plot_left_idx, const uint8_t *ref, const int64_t *ref_off, const uint8_t *aln,
+                     const int64_t *aln_off, const int64_t *rp, const int64_t *rp_off, const int64_t *matrix, int32_t msize,
+                     int64_t cut_point, int64_t seq_len, const uint8_t *unedited, const int64_t *n_deleted, const int64_t *n_inserted,
+                     const int64_t *n_mutated, const int64_t *reads, const double *pct, int64_t chunk, int64_t *err, c2b_amino **out);
+void c2b_amino_free(c2b_amino *a);
+int64_t c2b_amino_n(const c2b_amino *a);                          /* groups */
+int64_t c2b_amino_bytes(const c2b_amino *a);                      /* summed length of the groups' aligned reads */
+const int64_t *c2b_amino_ref_lens(const c2b_amino *a);            /* per row: residues of its reference protein */
+/* the groups in order: aligned read g at seq[seq_off[g] .. seq_off[g+1]), its aligned reference at the same offsets of ref */
+int  c2b_amino_fetch(const c2b_amino *a, uint8_t *seq, uint8_t *ref, int64_t *seq_off, uint8_t *unedited, int64_t *n_deleted,
+                     int64_t *n_inserted, int64_t *n_mutated, int64_t *reads, double *pct);
+/* wall time of the row pass with its copies, the alignments with the pair dedup, and silent edits with grouping (ms); pairs */
+int  c2b_amino_timings(const c2b_amino *a, double *row_ms, double *align_ms, double *group_ms, int64_t *n_pairs);
+
 /* ---- paired-end merge mode (csrc/c2b_paired.cpp) ----
  * get_consensus_alignment_from_pairs (CRISPRessoCORE.py:829-985, get_greater_qual_nuc :801-826): the two mates' alignments to one
  * amplicon (aligned read, aligned amplicon, score, quality string of the read's bases) merged column by column into one aligned
